@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 Halo2/KZG proving path.
+"""bench.py -- headline benchmark of the H100 Halo2/KZG proving path.
 
-BASELINE.json's metric has three terms: "SuperCircuit k=20 proof-gen sec + MSM G1-adds/s + NTT Fr-butterflies/s @1/2/4/8 B200".
+BASELINE.json's metric has three terms: "SuperCircuit k=20 proof-gen sec + MSM G1-adds/s + NTT Fr-butterflies/s @1/2/4/8 H100".
 The JSON line's `metric`/`value` is the FIRST term: wall-clock seconds of one create_proof (halo2 KZG + SHPLONK, Blake2b transcript)
 of the SuperCircuit-shaped k = 20 stand-in (tests/standins.py: 3 phases, 128 advice columns, 640 condition*constraint gates, 16
 lookup arguments = 48 input sets, 49 permutation columns incl. the instance column; the real circuit cannot be synthesised without
@@ -18,6 +18,10 @@ cpu_baseline objects: `ntt_2^24_round_trip` (configs[1]) and `msm_2^20` (configs
           cores; the Rust crate cannot be built here) on a BOUNDED sample of the same shape (smaller k), scaled linearly in the rows.
 
 Every proof timed here is checked AFTER the timed region by the pinned oracle verifier (`verified`), never inside it.
+
+  --dump-outputs DIR   after the timed steps, write the proof bytes of the last timed step of each headline path (one uint8 per
+          element, stored as float64) to DIR/proof_device_witness.npy and DIR/proof_host_witness.npy.  The inputs are seeded, so
+          two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -40,6 +44,8 @@ BUTTERFLIES_PER_DIR = (N_PTS // 2) * LOG_N          # 201,326,592  (SURVEY.md 8d
 ALG_BYTES_PER_DIR = 2 * 32 * N_PTS                  # 1,073,741,824 B: read + write each element once per transform
 MSM_LOG_N = 20
 SRS_S = 1234                                        # zkevm-circuits/src/super_circuit/test.rs:74 uses the same toy trapdoor
+HBM_PEAK_GBS = 3350.0
+HBM_PEAK_SOURCE = "NVIDIA H100 SXM data sheet (3.35 TB/s HBM3), not a measured figure"
 
 
 def dist_env():
@@ -50,11 +56,22 @@ def config_dict(world):
     return {"workload": f"create_proof of the SuperCircuit-shaped stand-in at k={K_PROOF}, {ADVICE} advice columns (BASELINE configs[3]); "
                         "N>1: the same single proof spread over N GPUs",
             "k": K_PROOF, "advice_columns": ADVICE, "transcript": "blake2b",
-            "l2": "working set (GBs of columns per stage) >> 126 MB L2: no flush needed", "n_gpus": world}
+            "l2": "working set (GBs of columns per stage) >> 50 MB L2: no flush needed", "n_gpus": world}
+
+
+def gpu_card(index):
+    """name, power limit and maximum SM clock of the card the numbers were measured on (nvidia-smi query)"""
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits", "-i", str(index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip().split(",")
+        return {"name": out[0].strip(), "power_limit_w": float(out[1]), "sm_max_mhz": float(out[2])}
+    except Exception as e:
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "query_error": repr(e)}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (recipe in B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,utilization.gpu"
 
@@ -370,6 +387,7 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-extras", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="write the proofs of the last timed steps as DIR/<name>.npy")
     ap.add_argument("--cpu-proof-child", nargs=2, type=int, default=None, help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.cpu_proof_child:
@@ -415,13 +433,17 @@ def main():
     if rank == 0:
         sampler.start()
     ctx.prof_enable(False)
-    sec_dev, _ = time_steps(prove_dev, W, K, barrier)
+    sec_dev, proof_dev = time_steps(prove_dev, W, K, barrier)
     sec_dev = max_over_ranks(sec_dev)
     launches0 = ctx.launch_count
     sec_e2e, proof = time_steps(prove_host, 1, K, barrier)
     sec_e2e = max_over_ranks(sec_e2e)
     launches = (ctx.launch_count - launches0) // K
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, p in (("proof_device_witness", proof_dev), ("proof_host_witness", proof)):
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), np.frombuffer(p, dtype=np.uint8).astype(np.float64))
     # per-kernel-class device time of ONE more proof (event pairs on the launching stream; outside the timed region because the
     # extra event records would perturb it)
     ctx.prof_enable(True)
@@ -431,13 +453,7 @@ def main():
     prof = {nm: ctx.prof_read(i) for i, nm in enumerate(names)}
     ctx.prof_enable(False)
     acct = proof_accounting(sc.shape, prof)
-    sc_shape_degree = sc.shape["cs_degree"]
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs_sustained", peaks.get("hbm_gbs", 6650.0)))
+    peak = HBM_PEAK_GBS
     kernels = {}
     for nm in names:
         cnt, ms = prof[nm]
@@ -448,30 +464,10 @@ def main():
                        "alg_bytes_per_proof": acct[nm]["alg_bytes"], "alg_units": acct[nm]["units"],
                        "achieved_gbs": per_launch_bytes / (ms / cnt * 1e-3) / 1e9}
     dom = max(kernels, key=lambda nm: kernels[nm]["ms_per_proof"])
-    # dram bytes per launch of the dominant kernel from the committed ncu --set full capture of this command (profiles/), if present
-    traffic, traffic_note = None, None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "r02_proof_k20_traffic.json")))
-        per = tj.get(dom, {}).get("dram_bytes_per_launch")
-        if per and dom == "expr_kernel":
-            # the ncu capture is one QUOTIENT launch (one coset part); the class also holds the small value-domain programs (lookup
-            # compression, permutation / grand-sum terms), so express it per average launch of the class like `achieved`
-            parts = 8 if sc_shape_degree == 9 else 4
-            traffic = parts * per / kernels[dom]["launches_per_proof"]
-            traffic_note = (f"{parts} quotient launches x {per / 1e9:.1f} GB (ncu --set full, profiles/r02_expr_kernel_k20_ncu.txt) / "
-                            f"{kernels[dom]['launches_per_proof']} launches of the class; algorithmic = {acct[dom]['alg_bytes'] / parts / 1e9:.1f} GB per quotient launch: the "
-                            "interpreter re-reads a column at every use and its local-memory register file competes for L2 (DESIGN.md 3.4)")
-        elif per:
-            traffic = per
-            traffic_note = "dram bytes of one launch (ncu --set full, profiles/)"
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "kernel": dom, "achieved": kernels[dom]["achieved_gbs"], "peak": peak, "unit": "GB/s",
-                "frac": kernels[dom]["achieved_gbs"] / peak,
-                "peak_source": "MEASURED_PEAKS.json (sustained copy bandwidth: the kernel runs inside a long step)" if peaks else "fallback 6650 GB/s",
-                "traffic": traffic, "traffic_note": traffic_note,
+                "frac": kernels[dom]["achieved_gbs"] / peak, "peak_source": HBM_PEAK_SOURCE, "traffic": None,
                 "note": "dominant kernel of the proof by measured device time; all three hot kernels are bound by the integer-multiply pipe "
-                        "(254-bit Montgomery arithmetic), not by HBM: see DESIGN.md section 2 and profiles/r02_microbench_pipes.txt",
+                        "(254-bit Montgomery arithmetic), not by HBM: see DESIGN.md section 2",
                 "kernels": kernels}
     vk_bytes = pk.vk_bytes()      # collective when world > 1: every rank calls it
     verdict = verify_with_oracle(sc, vk_bytes, proof, inst_h, fixed_h, sigma_h) if rank == 0 else None
@@ -500,7 +496,7 @@ def main():
     # ------------------------------------------------------------------ extras
     if not args.no_extras and world == 1:
         try:
-            extras["ntt_2^24_round_trip"] = bench_ntt(ctx, A, peak, peaks, args)
+            extras["ntt_2^24_round_trip"] = bench_ntt(ctx, A, peak, args)
         except Exception as e:
             extras["ntt_error"] = repr(e)
         try:
@@ -554,7 +550,8 @@ def main():
                 "dtype": "u256 (8x u32 Montgomery limbs, BN254 Fr/Fq)", "data": "synthetic (seeded satisfying witness of the stand-in; see tests/standins.py)",
                 "config": config_dict(world),
                 "e2e": {"value": sec_e2e, "unit": UNIT, "ms_per_step": sec_e2e * 1e3, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": len(proof)},
-                "gpu_launches": launches * K, "roofline": roofline, "cpu_baseline": cpu_baseline, "clocks": clocks, "extras": extras}
+                "gpu_launches": launches * K, "roofline": roofline, "cpu_baseline": cpu_baseline, "gpu": gpu_card(local_rank), "clocks": clocks,
+                "extras": extras}
         if failures:
             line["failures"] = failures
         print(json.dumps(line), flush=True)
@@ -564,7 +561,7 @@ def main():
         sys.exit(1)
 
 
-def bench_ntt(ctx, A, peak, peaks, args):
+def bench_ntt(ctx, A, peak, args):
     """BASELINE configs[1]: 2^24 Fr NTT forward + inverse round trip, data resident in HBM; e2e through the host-pointer entry point"""
     import numpy as np
     import torch
@@ -608,16 +605,12 @@ def bench_ntt(ctx, A, peak, peaks, args):
     assert torch.equal(host, orig.cpu()), "e2e round trip does not restore the input"
     passes = launches // (2 * K)
     avg_launch_s = ms_total * 1e-3 / launches
-    burst = float(peaks.get("hbm_gbs", peak))
     achieved = (ALG_BYTES_PER_DIR / passes) / avg_launch_s / 1e9
     out = {"butterflies_per_s": 2 * BUTTERFLIES_PER_DIR / (ms_step * 1e-3), "ms_per_round_trip": ms_step, "gpu_launches": launches,
            "e2e": {"butterflies_per_s": 2 * BUTTERFLIES_PER_DIR / (e2e_ms * 1e-3), "ms_per_round_trip": e2e_ms, "h2d_bytes_per_step": 2 * 32 * N_PTS,
                    "d2h_bytes_per_step": 2 * 32 * N_PTS},
-           "roofline": {"bound": "hbm", "kernel": "ntt_tile_kernel", "launches_per_transform": passes, "achieved": achieved, "peak": burst, "unit": "GB/s",
-                        "frac": achieved / burst, "alg_bytes_per_launch": ALG_BYTES_PER_DIR / passes,
-                        "traffic": 1213.4e6,
-                        "traffic_note": "dram read+write per launch, mean of the three passes of a transform (ncu --set full, profiles/r02_ntt_tile_v5_ncu.txt: "
-                                        "1586 / 1026 / 1031 MB; pass 1 also reads the 537 MB boundary-twiddle table)"}}
+           "roofline": {"bound": "hbm", "kernel": "ntt_tile_kernel", "launches_per_transform": passes, "achieved": achieved, "peak": peak, "unit": "GB/s",
+                        "frac": achieved / peak, "peak_source": HBM_PEAK_SOURCE, "alg_bytes_per_launch": ALG_BYTES_PER_DIR / passes, "traffic": None}}
     if not args.no_cpu_baseline:
         orc = load_oracle()
         a = orig.cpu().numpy().view(np.uint64).copy()
@@ -668,7 +661,7 @@ def bench_msm(ctx, A, peak, args):
            "commitment": r.compressed.hex(),
            "roofline": {"bound": "hbm", "kernel": "msm_acc_chunk_kernel", "achieved": n * 96 / (ms_acc / max(cnt, 1) * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                         "frac": n * 96 / (ms_acc / max(cnt, 1) * 1e-3) / 1e9 / peak, "alg_bytes_per_launch": n * 96, "avg_launch_ms": ms_acc / max(cnt, 1),
-                        "traffic": None, "note": "bucket accumulation is bound by the integer-multiply pipe (87.6 % fmaheavy, profiles/r02_msm_kernels_ncu.txt)"}}
+                        "peak_source": HBM_PEAK_SOURCE, "traffic": None, "note": "bucket accumulation is bound by the integer-multiply pipe"}}
     if not args.no_cpu_baseline:
         orc = load_oracle()
         hs, hb = scal.cpu().numpy().view(np.uint64), bases.cpu().numpy().view(np.uint64)

@@ -1,5 +1,5 @@
 /*
- * zkb200.h -- C ABI of libzkb200.so, the B200 (sm_100a) Halo2/KZG proving backend.
+ * zkb200.h -- C ABI of libzkb200.so, the H100 (sm_90a) Halo2/KZG proving backend.
  *
  * This is the boundary a fork-shaped `halo2_proofs` crate binds to (SURVEY.md section 8b): the reference swaps its
  * prover backend at crate level (docker/testool/gpu/Dockerfile:7, cargo `paths` override of halo2_proofs), and the
@@ -111,7 +111,7 @@ ZKB_API int32_t zkb_g1_fixed_base_mul_dev(zkb_ctx *ctx, const uint64_t base_affi
  * `downsize`s it for smaller circuits (prover/src/common/prover.rs:54-55, aggregator/src/recursion/util.rs:156).
  * zkb_srs_load       upload g / g_lagrange (2^k x 64 B each, halo2curves G1Affine layout) ONCE per context; g_lagrange may be
  *                    NULL: it is then derived on the device by the inverse FFT over G1 (`g_to_lagrange`).  Memory permitting
- *                    (ZKB_MSM_SHIFT_GB, default 24) the window-shifted copies 2^(c w) P_i of both bases are built, which turns
+ *                    (ZKB_MSM_SHIFT_GB, default 1/8 of device memory) the window-shifted copies 2^(c w) P_i of both bases are built, which turns
  *                    every commitment into ONE bucket set with no Horner pass (msm.cu).
  * zkb_srs_downsize   ParamsKZG::downsize(new_k): g truncated to 2^new_k, g_lagrange recomputed; the source handle stays valid.
  * zkb_srs_commit_*   ParamsKZG::commit (basis 0, coefficients against g) / commit_lagrange (basis 1, values against g_lagrange);

@@ -1,5 +1,5 @@
-// pipes.cu -- B200 micro-benchmarks that decide the next multiplier formulation (DESIGN.md 8c items 1 and 3).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipes pipes.cu && ./pipes
+// pipes.cu -- H100 micro-benchmarks that decide the next multiplier formulation (DESIGN.md section 9, item 1).
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipes pipes.cu && ./pipes
 // Measures, per SM sub-partition, cycles per warp instruction for:
 //   (a) IMAD.WIDE.U32 carry chains at ILP 1/2/4/8          -> dependent-issue latency and pipe throughput of the integer multiplier
 //   (b) DFMA chains at ILP 1/2/4/8                          -> same for the FP64 pipe

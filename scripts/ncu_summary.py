@@ -1,5 +1,5 @@
 """Summarise an .ncu-rep (read on the CPU box with `ncu -i`) into the handful of metrics DESIGN.md / bench.py cite.
-usage: python scripts/ncu_summary.py gpurun_out/prof.ncu-rep > profiles/rNN_name.txt"""
+usage: python scripts/ncu_summary.py prof.ncu-rep > summary.txt"""
 import csv, subprocess, sys
 
 WANT = [

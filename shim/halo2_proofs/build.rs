@@ -1,4 +1,4 @@
-// build.rs of the fork-shaped halo2_proofs: link the B200 backend.  Not compiled in this repository's image (no cargo).
+// build.rs of the fork-shaped halo2_proofs: link the H100 backend.  Not compiled in this repository's image (no cargo).
 fn main() {
     let dir = std::env::var("ZKB200_LIB_DIR").expect("set ZKB200_LIB_DIR to the directory holding libzkb200.so");
     println!("cargo:rustc-link-search=native={dir}");

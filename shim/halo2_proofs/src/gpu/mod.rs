@@ -1,4 +1,4 @@
-//! Process-global B200 context and caches.  Callers of the reference serialise proving behind a `Mutex<Prover>`
+//! Process-global H100 context and caches.  Callers of the reference serialise proving behind a `Mutex<Prover>`
 //! (prover/src/test/inner.rs:20-30) and may call from any thread, so the context is lazily created once and guarded by a mutex;
 //! one proof at a time per device, exactly as the library requires.  There is NO CPU fallback: a missing device is an error.
 pub mod csf;
@@ -22,7 +22,7 @@ pub fn gpu() -> std::sync::MutexGuard<'static, Gpu> {
     GPU.get_or_init(|| {
         let device: i32 = std::env::var("ZKB200_DEVICE").ok().and_then(|v| v.parse().ok()).unwrap_or(0);
         let mut ctx = std::ptr::null_mut();
-        check(unsafe { zkb_init(device, &mut ctx) }).expect("libzkb200: no usable B200 (there is no CPU fallback)");
+        check(unsafe { zkb_init(device, &mut ctx) }).expect("libzkb200: no usable H100 (there is no CPU fallback)");
         Mutex::new(Gpu { ctx, srs_by_k: HashMap::new(), pk_by_vk: HashMap::new() })
     })
     .lock()

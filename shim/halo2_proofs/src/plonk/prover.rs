@@ -1,4 +1,4 @@
-//! `plonk::create_proof` on the B200 proving session.  Same signature, same transcript traffic, same RNG draws as the CPU crate
+//! `plonk::create_proof` on the H100 proving session.  Same signature, same transcript traffic, same RNG draws as the CPU crate
 //! (halo2_proofs 1.1.0 @ e5ddf67 src/plonk/prover.rs); called unchanged from circuit-benchmarks/src/super_circuit.rs:117-132,
 //! circuit-benchmarks/src/packed_multi_keccak.rs:72-87 and, through snark-verifier-sdk, prover/src/common/prover/utils.rs:31.
 //!

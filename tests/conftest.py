@@ -7,7 +7,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")

@@ -1,5 +1,5 @@
 """Multi-GPU paths on real GPUs (skipped on a single-GPU box): domain-sharded NTT, point-range sharded MSM and the
-multi-GPU create_proof must reproduce the single-GPU results exactly.  Run under `gpurun --gpus 2`."""
+multi-GPU create_proof must reproduce the single-GPU results exactly.  Run on a machine with at least two GPUs."""
 import json
 import os
 import subprocess

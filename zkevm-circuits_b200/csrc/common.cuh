@@ -67,7 +67,8 @@ struct zkb_ctx {
     int device = 0;
     cudaStream_t stream = nullptr;
     cudaStream_t copy_stream = nullptr;  // H2D of witness columns overlaps the MSMs of the previous batch
-    int sm_count = 148;
+    int sm_count = 132;
+    size_t mem_bytes = 0;   // device memory (cudaDeviceProp::totalGlobalMem): the default budgets of the optional caches scale with it
     // multi-GPU: NCCL communicator of this rank (comm.cu); nranks == 1 -> everything local
     void *nccl_comm = nullptr;
     int rank = 0, nranks = 1;

@@ -88,13 +88,14 @@ extern "C" int32_t zkb_init(int32_t device, zkb_ctx **out) {
     ZKB_CUDA(cudaSetDevice(device));
     cudaDeviceProp prop;
     ZKB_CUDA(cudaGetDeviceProperties(&prop, device));
-    if (prop.major < 10) {
-        set_error("device %d is sm_%d%d; this library is built for sm_100a only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) {   // sm_90a code runs on compute capability 9.0 only
+        set_error("device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
         return ZKB_ERR_CUDA;
     }
     zkb_ctx *ctx = new zkb_ctx();
     ctx->device = device;
     ctx->sm_count = prop.multiProcessorCount;
+    ctx->mem_bytes = prop.totalGlobalMem;
     ZKB_CUDA(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking));
     ZKB_CUDA(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
     *out = ctx;

@@ -1,7 +1,6 @@
 // expr.cu -- device interpreter for constraint-expression programs (see expr.cuh).
 #include "common.cuh"
 #include "expr.cuh"
-#include <stdlib.h>
 
 namespace zkb {
 
@@ -17,9 +16,9 @@ struct ExprLaunch {
 };
 
 // Register file of the interpreter.  SMEM = true: in SHARED memory, two 16-byte planes indexed [reg][thread] (adjacent lanes touch
-// adjacent 16-byte slots: conflict free).  The first version kept it in local memory: 512 B per thread x ~150 k resident threads is
-// L2-sized, so the "registers" and the column data evicted each other and one coset part of the k = 20 quotient moved 107 GB
-// through HBM for 7.8 GB of algorithmic traffic (profiles/r02_expr_kernel_k20_ncu.txt).  SMEM = false: local memory (NREGS = 64).
+// adjacent 16-byte slots: conflict free).  SMEM = false: local memory, 512 B per thread at NREGS = 16: with every SM full that is
+// more than the L2 holds, so the "registers" and the column data evict each other and the DRAM traffic is a multiple of the
+// algorithmic one.
 template <int NREGS, int THREADS, bool SMEM>
 struct RegFile {
     uint4 *lo, *hi;
@@ -98,16 +97,13 @@ int32_t expr_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int n
     const uint32_t n = 1u << log_n;
     const unsigned blocks = (n + 127) / 128;
     ProfScope ps_(ctx, PROF_EXPR, st);
-    // Register file placement, measured on the k = 20 quotient (profiles/r02_expr_kernel_k20_ncu.txt, _smem_ncu.txt):
-    //   local memory, 16 registers : 65 ms per coset part, 107 GB of DRAM traffic (registers and columns evict each other from L2), pipe 75 %
-    //   shared memory, 16 registers: 92 ms per part,  12.6 GB of DRAM traffic (1.6x algorithmic) -- but 64 KB per 128 threads leaves 12
-    //                                warps per SM and the multiplier pipe drops to 52 %
-    // so programs of <= 8 registers (32 KB per block, 7 blocks per SM) run from shared memory, larger ones from local memory unless
-    // ZKB_EXPR_SMEM_REGS=1 asks for the low-traffic variant; the hybrid (8 registers in shared memory, the rest local) is the next step.
-    static const bool smem_regs = getenv("ZKB_EXPR_SMEM_REGS") && getenv("ZKB_EXPR_SMEM_REGS")[0] == '1';
+    // Register file placement: in local memory the registers and the columns compete for the 50 MB L2; in shared memory 16
+    // registers take 64 KB per 128 threads, which leaves 12 warps per SM.  On an H100 (80 GB SXM, 400 W power limit) the k = 20
+    // quotient program (9-16 registers) is faster from shared memory: 1.00 s instead of 1.18 s of interpreter time per proof,
+    // and the lower DRAM traffic lets the power-capped card hold higher clocks.  Programs of <= 16 registers therefore run from
+    // shared memory (32 KB per block for <= 8 registers), larger ones from local memory.
     if (nregs <= 8) ZKB_TRY((launch_smem<8, 128>(L, n, st)));
-    else if (nregs <= 16 && smem_regs) ZKB_TRY((launch_smem<16, 128>(L, n, st)));
-    else if (nregs <= 16) expr_kernel<16, 128, false><<<blocks, 128, 0, st>>>(L);
+    else if (nregs <= 16) ZKB_TRY((launch_smem<16, 128>(L, n, st)));
     else expr_kernel<64, 128, false><<<blocks, 128, 0, st>>>(L);
     ctx->launches++;
     ZKB_CUDA(cudaGetLastError());

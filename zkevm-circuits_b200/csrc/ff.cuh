@@ -1,4 +1,4 @@
-// ff.cuh -- 254-bit prime-field arithmetic for BN254 (Fr and Fq), host + device, sm_100a.
+// ff.cuh -- 254-bit prime-field arithmetic for BN254 (Fr and Fq), host + device, sm_90a.
 //
 // In-memory layout is exactly halo2curves' (scroll-tech/halo2curves @ a495a7b, src/bn256/{fr,fq}.rs):
 // 4 x u64 little-endian limbs of a*R mod p with R = 2^256, i.e. 8 x u32 little-endian limbs here.  Elements

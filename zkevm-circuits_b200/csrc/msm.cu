@@ -1,11 +1,11 @@
-// msm.cu -- multi-scalar multiplication over BN254 G1 (Pippenger bucket method) for sm_100a.
+// msm.cu -- multi-scalar multiplication over BN254 G1 (Pippenger bucket method) for sm_90a.
 //
 // Replaces halo2_proofs::arithmetic::best_multiexp (halo2_proofs 1.1.0 @ e5ddf67 src/arithmetic.rs), the body of
 // ParamsKZG::commit / commit_lagrange (src/poly/kzg/commitment.rs) -- every commitment of create_proof
 // (circuit-benchmarks/src/super_circuit.rs:117-132).  Same contract: sum_i coeffs[i] * bases[i]; the group element is
 // unique, so the normalised (affine / compressed) output is bit-identical to the CPU prover's.
 //
-// B200 design (NOT upstream's per-thread serial windows):
+// Design (NOT upstream's per-thread serial windows):
 //   1. scalars leave Montgomery form once and are recoded into signed c-bit digits (W = ceil(255/c) windows, buckets
 //      1..2^(c-1) per window) -- coalesced 32-byte loads, one thread per scalar;
 //   2. a counting sort (histogram -> scan -> scatter) groups point indices by (window, |digit|): 4 bytes per
@@ -541,7 +541,7 @@ int32_t msm_g1_batch_device_ex(zkb_ctx *ctx, const Fr *const *d_scalar_cols, uin
         uint64_t bound = (n * (shifted ? windows1 : 1) + CHUNK - 1) / CHUNK + 1;   // partials of the fullest possible bucket
         const uint32_t nscan = (uint32_t)(((uint64_t)nbuckets + SCAN_BLK - 1) / SCAN_BLK);
         const uint32_t *stw = (const uint32_t *)d_state;
-        const unsigned lv_blocks = (unsigned)std::min<uint64_t>((part0_n / ACC_CH + nbuckets + 127) / 128, 148ull * 32);
+        const unsigned lv_blocks = (unsigned)std::min<uint64_t>((part0_n / ACC_CH + nbuckets + 127) / 128, (uint64_t)ctx->sm_count * 32);
         while (bound > 1) {
             level_task_count_kernel<<<bb, 256, 0, st>>>(L, nbuckets);
             scan_blocks_gated_kernel<<<nscan, SCAN_T, 0, st>>>(tcount, toff[0], toff[1], stw, scan_tmp, nbuckets);

@@ -1,10 +1,10 @@
-// ntt.cu -- radix-2 NTT over BN254 Fr for sm_100a: persistent CTAs, TMA-staged data and twiddle tiles, mbarrier pipeline.
+// ntt.cu -- radix-2 NTT over BN254 Fr for sm_90a: persistent CTAs, TMA-staged data and twiddle tiles, mbarrier pipeline.
 //
 // Replaces halo2_proofs::arithmetic::best_fft (halo2_proofs 1.1.0 @ e5ddf67 src/arithmetic.rs; reached from
 // circuit-benchmarks/src/super_circuit.rs:117-132 through EvaluationDomain::{lagrange_to_coeff, coeff_to_extended,
 // extended_to_coeff}).  Same contract: in place, natural order in / natural order out, a'[k] = sum_j a[j] w^(jk).
 //
-// B200 design (NOT upstream's bit-reverse + log n global layers):
+// Design (NOT upstream's bit-reverse + log n global layers):
 //   n = A1 * A2 (* A3): 1 pass up to 2^11, 2 passes up to 2^20, 3 passes above (non-final factors <= 2^9, final <= 2^11).  A pass
 //   is ONE persistent kernel, TWO 256-thread CTAs per SM, each walking over TILES of 2048 elements (64 KB): a tile is C = 2048 / A
 //   adjacent columns of the Cooley-Tukey index split, i.e. C independent length-A transforms whose rows are C*32 contiguous bytes
@@ -33,9 +33,8 @@
 
 namespace zkb {
 
-// Measured on B200 (profiles/r02_ntt_tile_v5*_ncu.txt): two 256-thread CTAs per SM on 2048-element tiles reach 70 % of the
-// integer-multiply pipe; four 128-thread CTAs on 1024-element tiles do NOT do better (69 %): the four instruction streams of a
-// 440 KB kernel start to miss the instruction cache (stall_no_instruction 13 % of the samples vs 2 %).
+// Two 256-thread CTAs per SM on 2048-element tiles: a non-final pass takes 105 KB of shared memory per CTA (header + data tile
+// + twiddle ring + local twiddles), so two CTAs fit the 228 KB of an H100 SM.
 constexpr int NTT_TILE_BITS = 11;        // 2048 elements = 64 KB per tile
 constexpr int NTT_MAX_BITS = 11;         // largest in-CTA transform (final pass: no twiddle ring in shared memory)
 constexpr int NTT_PREF_INNER_BITS = 9;   // non-final passes: <= 8 KB of local twiddles next to the 32 KB twiddle ring -> two CTAs per SM

@@ -1,4 +1,4 @@
-// poly.cu -- polynomial utilities of the prover around MSM/NTT (SURVEY.md section 8a rows a5-a9), sm_100a.
+// poly.cu -- polynomial utilities of the prover around MSM/NTT (SURVEY.md section 8a rows a5-a9), sm_90a.
 //
 //   fr_powers            : out[i] = base^i                  (coset scaling tables, omega^i for the permutation argument)
 //   poly_eval (batched)  : halo2_proofs::arithmetic::eval_polynomial over many polynomials at one point (row a8)

@@ -14,7 +14,7 @@
 // vk.transcript_repr (Rust-specific derivations, SURVEY.md hard part 1).  Everything else stays in HBM: columns,
 // polynomials, coset evaluations, the quotient; only 64-byte commitments and 32-byte evaluations return to the host.
 //
-// B200 design points (not upstream's): the quotient is evaluated coset-part by coset-part (extended domain = E cosets of
+// Design points (not upstream's): the quotient is evaluated coset-part by coset-part (extended domain = E cosets of
 // size n, SURVEY 8e) by ONE fused interpreter kernel per part; all scans / inversions / evaluations are parallel kernels.
 #include "common.cuh"
 #include "expr.cuh"
@@ -560,13 +560,14 @@ static int32_t pk_build(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, c
     ZKB_TRY(lagrange_to_coeff(pk.get(), pk->lblind_poly, pk->lblind_poly, st));
     ZKB_TRY(fr_powers_device(ctx, pk->omega, n, pk->omega_pows, st));
     {
-        // cache the coset evaluations of the static polynomials unless that would take more than ZKB_COSET_CACHE_GB (default 48)
+        // cache the coset evaluations of the static polynomials unless that would take more than ZKB_COSET_CACHE_GB (default: a
+        // quarter of the device memory, 20 GB on an 80 GB H100 -- the rest holds the proving session's columns and coset parts)
         std::vector<Fr *> stat;
         for (auto q : pk->fixed_polys) stat.push_back(q);
         for (auto q : pk->sigma_polys) stat.push_back(q);
         stat.push_back(pk->l0_poly); stat.push_back(pk->llast_poly); stat.push_back(pk->lblind_poly); stat.push_back(pk->xid_poly);
         const char *env = getenv("ZKB_COSET_CACHE_GB");
-        const double budget = (env ? atof(env) : 48.0) * 1e9;
+        const double budget = env ? atof(env) * 1e9 : 0.25 * (double)ctx->mem_bytes;
         if ((double)stat.size() * pk->N * sizeof(Fr) <= budget) {
             Fr *pows = nullptr;
             ZKB_TRY(pk->pool.fr(n, &pows));

@@ -8,7 +8,7 @@
 // chain here: log n radix-2 stages on XYZZ points, each butterfly one scalar multiplication by a twiddle.
 //
 // One zkb_srs per context is shared by every proving key created from it (zkb_pk_create_with_srs): the 64-byte bases are
-// uploaded once, and -- memory permitting (ZKB_MSM_SHIFT_GB, default 24) -- the window-shifted copies 2^(c w) P_i used by the
+// uploaded once, and -- memory permitting (ZKB_MSM_SHIFT_GB, default an eighth of the device memory) -- the window-shifted copies 2^(c w) P_i used by the
 // one-bucket-set Pippenger variant are built once.
 #include "common.cuh"
 #include <stdlib.h>
@@ -104,11 +104,12 @@ static void srs_free(zkb_srs *s) {
     for (auto &b : s->blocks) block_free(s->ctx, b.first, b.second);
     delete s;
 }
-// window-shifted copies unless they would exceed ZKB_MSM_SHIFT_GB (default 24) in total
+// window-shifted copies unless they would exceed ZKB_MSM_SHIFT_GB (default: an eighth of the device memory, 10 GB on an 80 GB
+// H100) in total
 static int32_t srs_build_shifted(zkb_srs *s, cudaStream_t st) {
     const uint32_t copies = msm_shift_copies(s->n);
     const char *env = getenv("ZKB_MSM_SHIFT_GB");
-    const double budget = (env ? atof(env) : 24.0) * 1e9;
+    const double budget = env ? atof(env) * 1e9 : 0.125 * (double)s->ctx->mem_bytes;
     if (copies && 2.0 * copies * s->n * sizeof(G1Affine) <= budget) {
         ZKB_TRY(srs_alloc(s, (size_t)copies * s->n * sizeof(G1Affine), (void **)&s->g_shift));
         ZKB_TRY(srs_alloc(s, (size_t)copies * s->n * sizeof(G1Affine), (void **)&s->g_lagrange_shift));

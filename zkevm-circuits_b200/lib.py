@@ -1,6 +1,6 @@
 """ctypes binding of libzkb200.so (the C ABI declared in include/zkb200.h).
 
-There is no CPU fallback: if the shared library is missing, or no sm_100 device is present, every compute entry
+There is no CPU fallback: if the shared library is missing, or no sm_90 (H100) device is present, every compute entry
 point raises ZkbError.  Build with `python -c "import __graft_entry__ as g; g.build()"` or `make -C zkevm-circuits_b200/csrc`.
 """
 import ctypes
