@@ -171,6 +171,12 @@ __global__ void counts_to_fr_kernel(const uint32_t *__restrict__ counts, uint32_
 
 // ---------------------------------------------------------------------------------------------------------- helpers
 static Fr fr_from_u64(uint64_t v) { return fp_from_u64<FrParams>(v); }
+// the permutation argument's DELTA = 7^(2^28): column i of a permutation set is labelled by DELTA^i
+static Fr perm_delta() {
+    Fr d = fr_from_u64(7);
+    for (int i = 0; i < 28; ++i) d = fp_sqr(d);
+    return d;
+}
 static bool fr_less(const Fr &a, const Fr &b) {  // halo2curves Ord: canonical integer comparison
     Fr x = fp_to_canonical(a), y = fp_to_canonical(b);
     for (int i = 7; i >= 0; --i) {
@@ -195,15 +201,14 @@ struct zkb_pk {
     Fr *l0_poly = nullptr, *llast_poly = nullptr, *lblind_poly = nullptr, *xid_poly = nullptr, *omega_pows = nullptr;
     zkb_srs *srs = nullptr;       // shared ParamsKZG handle (owned when the pk was made by the legacy zkb_pk_create)
     bool owns_srs = false;
-    G1Affine *g = nullptr, *g_lagrange = nullptr;   // = srs->g / srs->g_lagrange
     // coset evaluations of the proof-independent polynomials (fixed, sigma, l_0, l_last, l_blind, X) for every coset part,
     // like upstream's pk.fixed_cosets / permutation cosets / l0 / l_last / l_active_row: [part][poly] -> n elements
     std::vector<std::vector<Fr *>> coset_cache;
-    // window-shifted copies of the SRS (copy w = 2^(c w) * P_i) for the Pippenger variant with one bucket set per column (= srs->*_shift)
-    G1Affine *g_shift = nullptr, *g_lagrange_shift = nullptr;
     ~zkb_pk() {
         if (owns_srs && srs) zkb_srs_destroy(srs);
     }
+    // generator zeta * ext_omega^j of coset part j
+    Fr coset_gen(uint32_t j) const { return fp_mul(zeta, fp_pow_u64(ext_omega, j)); }
 };
 
 struct zkb_session {
@@ -251,6 +256,19 @@ template <class F>
 static void push_be32(std::vector<uint8_t> &dst, const F &canonical) {
     const uint8_t *b = (const uint8_t *)canonical.l;
     for (int i = 31; i >= 0; --i) dst.push_back(b[i]);
+}
+// Challenge255 squeeze of a Blake2b transcript: absorb the 0x00 prefix, then Fr::from_uniform_bytes of the 64-byte digest,
+// (lo + hi * 2^256) mod r, computed with Montgomery multiplications by R^2
+static Fr blake2b_challenge255(Blake2b &tr) {
+    const uint8_t pre = 0;
+    tr.update(&pre, 1);
+    uint8_t h[64];
+    tr.finalize_copy(h);
+    Fr lo, hi;
+    memcpy(lo.l, h, 32);
+    memcpy(hi.l, h + 32, 32);
+    const Fr r2 = Fr::r2();
+    return fp_add(fp_mul(lo, r2), fp_mul(fp_mul(hi, r2), r2));
 }
 static void tr_common_scalar(zkb_session *s, const Fr &v) {
     if (s->tkind == 3) { const int32_t r = s->vt.common_scalar(s->vt.user, (const uint64_t *)v.l); if (r && !s->cb_error) s->cb_error = r; return; }
@@ -316,41 +334,30 @@ static Fr tr_squeeze(zkb_session *s) {
         for (int i = 0; i < 32; ++i) b[i] = h[31 - i];
         return fp_mul(v, Fr::r2());  // Montgomery multiply reduces any 256-bit value: v * R^2 / R = v R mod r
     }
-    const uint8_t pre = 0;
-    s->tr.update(&pre, 1);
-    uint8_t h[64];
-    s->tr.finalize_copy(h);
-    Fr lo, hi;
-    memcpy(lo.l, h, 32);
-    memcpy(hi.l, h + 32, 32);
-    // Fr::from_uniform_bytes: (lo + hi * 2^256) mod r, computed with Montgomery multiplications by R^2
-    const Fr r2 = Fr::r2();
-    return fp_add(fp_mul(lo, r2), fp_mul(fp_mul(hi, r2), r2));
+    return blake2b_challenge255(s->tr);
+}
+// first failure a caller's transcript callback reported (callbacks run inside the transcript operations, which return nothing)
+static int32_t callback_status(const zkb_session *s) {
+    if (s->cb_error) { set_error("the caller's transcript callback failed (%d)", s->cb_error); return ZKB_ERR_STATE; }
+    return ZKB_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------- basis changes
 static int32_t lagrange_to_coeff(zkb_pk *pk, const Fr *values, Fr *poly, cudaStream_t st) {
     return ntt_fr_device(pk->ctx, values, poly, pk->k, pk->omega_inv, &pk->n_inv, 0, nullptr, st);
 }
-static int32_t commit(zkb_pk *pk, const Fr *scalars, const G1Affine *bases, uint64_t len, G1Affine *out, cudaStream_t st) {
-    return msm_g1_device(pk->ctx, scalars, bases, len, out, st);
-}
-
-// commit several columns against the same bases with batched MSMs (one pass per <= msm_max_batch columns)
-static int32_t commit_many_local(zkb_pk *pk, const std::vector<Fr *> &cols, const G1Affine *bases, uint64_t len, std::vector<G1Affine> &out, cudaStream_t st) {
-    out.resize(cols.size());
-    const uint32_t maxb = msm_max_batch(len);
-    const G1Affine *shift = (bases == pk->g) ? pk->g_shift : (bases == pk->g_lagrange) ? pk->g_lagrange_shift : nullptr;
-    if (len != pk->n) shift = nullptr;
-    for (size_t done = 0; done < cols.size(); done += maxb) {
-        const uint32_t cur = (uint32_t)std::min<size_t>(maxb, cols.size() - done);
-        const Fr **d_tbl = nullptr;
-        ZKB_TRY(scratch_get(pk->ctx, SCR_MSM_TBL, 64 * sizeof(Fr *), (void **)&d_tbl));
-        ZKB_CUDA(cudaMemcpyAsync(d_tbl, cols.data() + done, cur * sizeof(Fr *), cudaMemcpyHostToDevice, st));
-        ZKB_TRY(msm_g1_batch_device_ex(pk->ctx, d_tbl, cur, shift ? shift : bases, len, out.data() + done, shift != nullptr, st));
+// size-n NTTs of many columns, batched in chunks that need at most 2 GiB of NTT scratch
+static int32_t ntt_many(zkb_pk *pk, const std::vector<Fr *> &src, const std::vector<Fr *> &dst, const Fr &w, const Fr *scale, const Fr *in_scale,
+                        cudaStream_t st) {
+    const uint32_t chunk = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(256, (1ull << 31) / (pk->n * sizeof(Fr))));
+    for (size_t done = 0; done < src.size(); done += chunk) {
+        const uint32_t cur = (uint32_t)std::min<size_t>(chunk, src.size() - done);
+        std::vector<Fr *> a(src.begin() + done, src.begin() + done + cur), b(dst.begin() + done, dst.begin() + done + cur);
+        ZKB_TRY(ntt_fr_batch_device(pk->ctx, a.data(), b.data(), cur, pk->k, w, scale, 0, in_scale, st));
     }
     return ZKB_OK;
 }
+
 // multi-GPU dealing of independent units (columns, lookup arguments, coset parts): the `count` units are cut into P contiguous
 // blocks of blk = ceil(count / P), rank r computes block r.  Results live in a slab of P * blk unit slots (the tail of the last
 // blocks is padding), so ONE in-place ncclAllGather (every rank contributes its own block, 1/P of the slab) completes it -- no
@@ -370,15 +377,28 @@ static int32_t deal_gather(zkb_ctx *ctx, const Deal &d, void *slab, size_t unit_
     if (!d.on) return ZKB_OK;
     return comm_allgather(ctx, (const uint8_t *)slab + (size_t)d.rank * d.blk * unit_bytes, slab, d.blk * unit_bytes, st);
 }
+// cols[i] = column i of a new slab of d.padded() columns of n elements (nothing is allocated for no columns)
+static int32_t dealt_columns(DevPool &pool, const Deal &d, uint64_t n, std::vector<Fr *> &cols, Fr **slab) {
+    cols.resize(d.count);
+    if (!d.count) return ZKB_OK;
+    ZKB_TRY(pool.fr(d.padded() * n, slab));
+    for (size_t i = 0; i < d.count; ++i) cols[i] = *slab + i * n;
+    return ZKB_OK;
+}
 
-// commit several columns against the same bases with batched MSMs.  With a communicator the columns are dealt in contiguous blocks
-// (Deal) and the 64-byte results are all-gathered.
-static int32_t commit_many(zkb_pk *pk, const std::vector<Fr *> &cols, const G1Affine *bases, uint64_t len, std::vector<G1Affine> &out, cudaStream_t st) {
+// srs_commit_many's basis index: g (coefficient form, ParamsKZG::commit) / g_lagrange (values, commit_lagrange)
+enum { BASIS_G = 0, BASIS_LAGRANGE = 1 };
+
+// commit several size-n columns against one basis with batched MSMs.  With a communicator the columns are dealt in contiguous
+// blocks (Deal) and the 64-byte results are all-gathered.
+static int32_t commit_many(zkb_pk *pk, const std::vector<Fr *> &cols, int basis, std::vector<G1Affine> &out, cudaStream_t st) {
     zkb_ctx *ctx = pk->ctx;
+    const uint64_t len = pk->n;
     if (ctx->nranks > 1 && cols.size() == 1 && len >= (1u << 14)) {
         // a single commitment (random polynomial, SHPLONK's h and the final quotient) cannot be dealt: shard it by point range instead
         // (SURVEY 8e): every rank reduces len / P points, the 64-byte partial sums are all-gathered and added on the host
         const uint64_t P = (uint64_t)ctx->nranks, lo = len * (uint64_t)ctx->rank / P, hi = len * ((uint64_t)ctx->rank + 1) / P;
+        const G1Affine *bases = basis == BASIS_G ? pk->srs->g : pk->srs->g_lagrange;
         G1Affine part;
         ZKB_TRY(msm_g1_device(ctx, cols[0] + lo, bases + lo, hi - lo, &part, st));
         G1Affine *d_buf = nullptr;
@@ -394,12 +414,15 @@ static int32_t commit_many(zkb_pk *pk, const std::vector<Fr *> &cols, const G1Af
         return ZKB_OK;
     }
     const Deal d(ctx, cols.size());
-    if (!d.on) return commit_many_local(pk, cols, bases, len, out, st);
+    if (!d.on) {
+        out.resize(cols.size());
+        return srs_commit_many(pk->srs, basis, cols.data(), (uint32_t)cols.size(), len, out.data(), st);
+    }
     std::vector<Fr *> mine;
     for (size_t i = 0; i < cols.size(); ++i)
         if (d.mine(i)) mine.push_back(cols[i]);
-    std::vector<G1Affine> part;
-    if (!mine.empty()) ZKB_TRY(commit_many_local(pk, mine, bases, len, part, st));
+    std::vector<G1Affine> part(mine.size());
+    if (!mine.empty()) ZKB_TRY(srs_commit_many(pk->srs, basis, mine.data(), (uint32_t)mine.size(), len, part.data(), st));
     G1Affine *d_buf = nullptr;
     ZKB_TRY(scratch_get(ctx, SCR_COMM, d.padded() * sizeof(G1Affine), (void **)&d_buf));
     if (!part.empty()) ZKB_CUDA(cudaMemcpyAsync(d_buf + (size_t)d.rank * d.blk, part.data(), part.size() * sizeof(G1Affine), cudaMemcpyHostToDevice, st));
@@ -408,6 +431,13 @@ static int32_t commit_many(zkb_pk *pk, const std::vector<Fr *> &cols, const G1Af
     ZKB_CUDA(cudaMemcpyAsync(out.data(), d_buf, d.padded() * sizeof(G1Affine), cudaMemcpyDeviceToHost, st));
     ZKB_CUDA(cudaStreamSynchronize(st));
     out.resize(cols.size());
+    return ZKB_OK;
+}
+// commit the columns and write the commitments to the transcript in order
+static int32_t commit_write(zkb_session *s, const std::vector<Fr *> &cols, int basis, cudaStream_t st) {
+    std::vector<G1Affine> cms;
+    ZKB_TRY(commit_many(s->pk, cols, basis, cms, st));
+    for (auto &cm : cms) ZKB_TRY(tr_write_point(s, cm));
     return ZKB_OK;
 }
 
@@ -435,9 +465,37 @@ static int32_t upload_table(DevPool &pool, const std::vector<T *> &host, T ***de
     ZKB_CUDA(cudaStreamSynchronize(st));
     return ZKB_OK;
 }
+// one program whose root i is STOREd to outs[i], uploaded with its output table and run over the n rows of the d_cols table
+static int32_t run_store_program(zkb_pk *pk, DevPool &pool, ExprBuilder &eb, const std::vector<uint32_t> &roots, const std::vector<Fr *> &outs,
+                                 const Fr *const *d_cols, const std::string &what, cudaStream_t st) {
+    ProgramBuilder pb(eb);
+    std::vector<ProgramBuilder::Root> stores;
+    for (size_t i = 0; i < roots.size(); ++i) stores.push_back({roots[i], ProgramBuilder::STORE, (uint32_t)i});
+    if (!pb.scope(stores)) { set_error("%s: %s", what.c_str(), pb.error.c_str()); return ZKB_ERR_ARG; }
+    DeviceProgram dp;
+    ZKB_TRY(upload_program(pool, pb, eb, dp, st));
+    Fr **d_outs = nullptr;
+    ZKB_TRY(upload_table(pool, outs, &d_outs, st));
+    return expr_run_device(pk->ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, pk->k, 1, 0, st);
+}
+// out (+)= sum_i coefs[i] * polys[i] over n coefficients.  `coefs` is copied asynchronously: keep it alive until the stream is synchronised.
+static int32_t lincomb(zkb_pk *pk, DevPool &pool, const std::vector<Fr *> &polys, const std::vector<Fr> &coefs, Fr *out, bool accumulate, cudaStream_t st) {
+    Fr **d_p = nullptr;
+    Fr *d_c = nullptr;
+    ZKB_TRY(upload_table(pool, polys, &d_p, st));
+    ZKB_TRY(pool.fr(coefs.size(), &d_c));
+    ZKB_CUDA(cudaMemcpyAsync(d_c, coefs.data(), coefs.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
+    return lincomb_device(pk->ctx, d_p, d_c, (uint32_t)polys.size(), pk->n, out, accumulate, st);
+}
 
-// translate CSF nodes into ExprBuilder nodes; column slot numbering is supplied by the caller
-struct SlotMap { uint32_t fixed0, advice0, instance0; };
+// column slots common to the value-domain and the coset-domain tables: [fixed | advice | instance | sigma | ...]
+struct SlotMap {
+    uint32_t fixed0, advice0, instance0, sigma0;
+    explicit SlotMap(const Csf &cs) : fixed0(0), advice0(cs.nf), instance0(cs.nf + cs.na), sigma0(cs.nf + cs.na + cs.ni) {}
+    // slot of a permutation column (kind, index)
+    uint32_t perm(const std::array<uint32_t, 2> &c) const { return c[0] == N_FIXED ? fixed0 + c[1] : c[0] == N_ADVICE ? advice0 + c[1] : instance0 + c[1]; }
+};
+// translate CSF nodes into ExprBuilder nodes
 static uint32_t translate(const Csf &cs, uint32_t node, ExprBuilder &eb, const SlotMap &sm, const std::vector<Fr> &challenges, std::vector<int64_t> &memo) {
     if (memo[node] >= 0) return (uint32_t)memo[node];
     const auto &nd = cs.nodes[node];
@@ -505,40 +563,23 @@ static int32_t pk_build(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, c
     pk->N_inv = fp_inv(fr_from_u64(pk->N));
     pk->zeta = host_zeta();
     pk->t_inv.resize(pk->E);
-    for (uint32_t j = 0; j < pk->E; ++j) {
-        Fr gj = fp_mul(pk->zeta, fp_pow_u64(pk->ext_omega, j));
-        pk->t_inv[j] = fp_inv(fp_sub(fp_pow_u64(gj, n), Fr::one()));
-    }
-    pk->g = srs->g;
-    pk->g_lagrange = srs->g_lagrange;
-    pk->g_shift = srs->g_shift;
-    pk->g_lagrange_shift = srs->g_lagrange_shift;
-    // fixed / sigma columns: values and coefficient form
-    auto ingest = [&](const uint64_t *const *src, size_t cnt, std::vector<Fr *> &vals, std::vector<Fr *> &polys) -> int32_t {
+    for (uint32_t j = 0; j < pk->E; ++j) pk->t_inv[j] = fp_inv(fp_sub(fp_pow_u64(pk->coset_gen(j), n), Fr::one()));
+    // fixed / sigma columns: values and coefficient form (sources on the host, or on the device for keygen's sigma)
+    auto ingest = [&](const void *const *src, size_t cnt, std::vector<Fr *> &vals, std::vector<Fr *> &polys) -> int32_t {
         vals.resize(cnt);
         polys.resize(cnt);
         for (size_t i = 0; i < cnt; ++i) {
             ZKB_TRY(pk->pool.fr(n, &vals[i]));
             ZKB_TRY(pk->pool.fr(n, &polys[i]));
-            ZKB_CUDA(cudaMemcpyAsync(vals[i], src[i], n * sizeof(Fr), cudaMemcpyHostToDevice, st));
+            ZKB_CUDA(cudaMemcpyAsync(vals[i], src[i], n * sizeof(Fr), cudaMemcpyDefault, st));
             ZKB_TRY(lagrange_to_coeff(pk.get(), vals[i], polys[i], st));
         }
         return ZKB_OK;
     };
-    ZKB_TRY(ingest(fixed_values, cs.nf, pk->fixed_values, pk->fixed_polys));
-    if (sigma_dev) {
-        ZKB_ARG(sigma_dev->size() == cs.perm.size());
-        pk->sigma_values.resize(cs.perm.size());
-        pk->sigma_polys.resize(cs.perm.size());
-        for (size_t i = 0; i < cs.perm.size(); ++i) {
-            ZKB_TRY(pk->pool.fr(n, &pk->sigma_values[i]));
-            ZKB_TRY(pk->pool.fr(n, &pk->sigma_polys[i]));
-            ZKB_CUDA(cudaMemcpyAsync(pk->sigma_values[i], (*sigma_dev)[i], n * sizeof(Fr), cudaMemcpyDeviceToDevice, st));
-            ZKB_TRY(lagrange_to_coeff(pk.get(), pk->sigma_values[i], pk->sigma_polys[i], st));
-        }
-    } else {
-        ZKB_TRY(ingest(sigma_values, cs.perm.size(), pk->sigma_values, pk->sigma_polys));
-    }
+    ZKB_TRY(ingest((const void *const *)fixed_values, cs.nf, pk->fixed_values, pk->fixed_polys));
+    if (sigma_dev) ZKB_ARG(sigma_dev->size() == cs.perm.size());
+    const void *const *sigma_src = sigma_dev ? (const void *const *)sigma_dev->data() : (const void *const *)sigma_values;
+    ZKB_TRY(ingest(sigma_src, cs.perm.size(), pk->sigma_values, pk->sigma_polys));
     // l_0, l_last, l_blind (Lagrange indicator vectors -> coefficient form), X (identity polynomial), omega^i
     ZKB_TRY(pk->pool.fr(n, &pk->l0_poly));
     ZKB_TRY(pk->pool.fr(n, &pk->llast_poly));
@@ -573,8 +614,7 @@ static int32_t pk_build(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, c
             ZKB_TRY(pk->pool.fr(n, &pows));
             pk->coset_cache.resize(pk->E);
             for (uint32_t j = 0; j < pk->E; ++j) {
-                const Fr gj = fp_mul(pk->zeta, fp_pow_u64(pk->ext_omega, j));
-                ZKB_TRY(fr_powers_device(ctx, gj, n, pows, st));
+                ZKB_TRY(fr_powers_device(ctx, pk->coset_gen(j), n, pows, st));
                 pk->coset_cache[j].resize(stat.size());
                 for (size_t i = 0; i < stat.size(); ++i) {
                     ZKB_TRY(pk->pool.fr(n, &pk->coset_cache[j][i]));
@@ -658,9 +698,7 @@ extern "C" int32_t zkb_keygen_pk(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf
     ZKB_CUDA(cudaMemcpyAsync(d_mr, map_row.data(), P * n * 4, cudaMemcpyHostToDevice, st));
     Fr omega = host_root_of_unity(cs.k);
     ZKB_TRY(fr_powers_device(ctx, omega, n, d_om, st));
-    Fr delta = fr_from_u64(7);
-    for (int i = 0; i < 28; ++i) delta = fp_sqr(delta);   // DELTA = 7^(2^28)
-    ZKB_TRY(fr_powers_device(ctx, delta, P + 1, d_dl, st));
+    ZKB_TRY(fr_powers_device(ctx, perm_delta(), P + 1, d_dl, st));
     std::vector<Fr *> sig(P);
     for (size_t c = 0; c < P; ++c) {
         ZKB_TRY(tmp.fr(n, &sig[c]));
@@ -750,15 +788,7 @@ extern "C" int32_t zkb_blake2b_challenge_host(const uint8_t *bytes, uint64_t len
     ZKB_ARG(out && (bytes || len == 0));
     Blake2b st("Halo2-Transcript");
     if (len) st.update(bytes, len);
-    const uint8_t pre = 0;
-    st.update(&pre, 1);
-    uint8_t h[64];
-    st.finalize_copy(h);
-    Fr lo, hi;
-    memcpy(lo.l, h, 32);
-    memcpy(hi.l, h + 32, 32);
-    const Fr r2 = Fr::r2();
-    const Fr c = fp_add(fp_mul(lo, r2), fp_mul(fp_mul(hi, r2), r2));
+    const Fr c = blake2b_challenge255(st);
     memcpy(out, c.l, 32);
     return ZKB_OK;
 }
@@ -779,7 +809,7 @@ extern "C" int32_t zkb_pk_vk_bytes(zkb_pk *pk, uint8_t *out, uint64_t cap, uint6
     for (auto c : pk->fixed_values) cols.push_back(c);
     for (auto c : pk->sigma_values) cols.push_back(c);
     std::vector<G1Affine> cms;
-    if (!cols.empty()) ZKB_TRY(commit_many(pk, cols, pk->g_lagrange, pk->n, cms, st));
+    if (!cols.empty()) ZKB_TRY(commit_many(pk, cols, BASIS_LAGRANGE, cms, st));
     auto be32 = [](uint8_t *p, uint32_t v) { p[0] = (uint8_t)(v >> 24); p[1] = (uint8_t)(v >> 16); p[2] = (uint8_t)(v >> 8); p[3] = (uint8_t)v; };
     be32(out, cs.k);
     be32(out + 4, cs.nf);
@@ -901,7 +931,7 @@ static int32_t prove_begin_common(zkb_pk *pk, int32_t transcript_kind, const zkb
     s->adv_values.assign(cs.na, nullptr);
     s->challenges.assign(cs.nch, Fr::zero());
     ZKB_CUDA(cudaStreamSynchronize(st));
-    if (s->cb_error) { set_error("the caller's transcript callback failed (%d)", s->cb_error); return ZKB_ERR_STATE; }
+    ZKB_TRY(callback_status(s.get()));
     *out = s.release();
     return ZKB_OK;
 }
@@ -968,10 +998,8 @@ extern "C" int32_t zkb_prove_advice_phase(zkb_session *s, uint32_t phase, const 
     for (size_t b = 0; b < nbatch; ++b) {
         ZKB_CUDA(cudaStreamWaitEvent(st, evs[b], 0));
         const size_t lo = dealt ? 0 : b * maxb, hi = dealt ? ncols : std::min(ncols, (b + 1) * (size_t)maxb);
-        std::vector<Fr *> part(phase_cols.begin() + lo, phase_cols.begin() + hi);
-        std::vector<G1Affine> cms;
-        ZKB_TRY(commit_many(pk, part, pk->g_lagrange, n, cms, st));   // dealt: the same contiguous blocks as the uploads (same unit count)
-        for (auto &cm : cms) ZKB_TRY(tr_write_point(s, cm));
+        // dealt: the same contiguous blocks as the uploads (same unit count)
+        ZKB_TRY(commit_write(s, std::vector<Fr *>(phase_cols.begin() + lo, phase_cols.begin() + hi), BASIS_LAGRANGE, st));
     }
     ZKB_TRY(deal_gather(pk->ctx, deal, slab, n * sizeof(Fr), st));   // column data of the other ranks' blocks over NVLink
     for (uint32_t i = 0; i < cs.nch; ++i) {
@@ -981,8 +1009,7 @@ extern "C" int32_t zkb_prove_advice_phase(zkb_session *s, uint32_t phase, const 
         }
     }
     s->next_phase++;
-    if (s->cb_error) { set_error("the caller's transcript callback failed (%d)", s->cb_error); return ZKB_ERR_STATE; }
-    return ZKB_OK;
+    return callback_status(s);
 }
 
 extern "C" int32_t zkb_session_destroy(zkb_session *s) {
@@ -1024,72 +1051,68 @@ struct OpenQuery {
     int poly_id;        // identity of the committed polynomial
     const Fr *poly;     // device coefficients (n)
     int64_t rot;        // point = x * omega^rot
-    Fr point;
-    Fr eval;
 };
 
-static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const uint64_t *phi_blinds, const uint64_t *random_poly_host) {
+// what one stage of the proof hands to a later one
+struct ProofState {
+    Fr theta, beta, gamma, y, x;
+    Fr **d_vcols = nullptr;                  // value-domain column table: [fixed | advice | instance | sigma | omega_pows]
+    std::vector<std::vector<Fr *>> lk_f;     // compressed inputs per lookup / input set
+    std::vector<Fr *> lk_t, lk_m;            // compressed table, multiplicities per lookup
+    std::vector<Fr *> zs, phis;              // permutation grand products per set, lookup grand sums per lookup
+    Fr *random_poly = nullptr;
+    std::vector<Fr *> adv_polys, z_polys, phi_polys, m_polys;
+    Fr *h_ext = nullptr;                     // h on the extended domain; after the inverse transform, qdeg pieces of n coefficients
+    std::vector<Fr *> h_pieces;
+    std::map<int64_t, Fr> point_of;          // rotation -> x * omega^rot
+    std::map<std::pair<int, int64_t>, Fr> eval_of;
+    std::vector<OpenQuery> queries;          // multiopen queries in prover.rs order
+};
+
+// mv_lookup/prover.rs prepare: theta, compressed inputs and table (interpreter on the Lagrange domain), multiplicities m over the
+// usable rows, m commitments.  Multi-GPU: the lookup arguments are dealt and the m columns, one slab, are all-gathered.
+static int32_t lookup_prepare(zkb_session *s, ProofState &ps) {
     zkb_pk *pk = s->pk;
     zkb_ctx *ctx = pk->ctx;
     const Csf &cs = pk->cs;
     const uint64_t n = pk->n;
-    const uint32_t bf = cs.bf, k = cs.k;
-    const uint32_t usable = (uint32_t)(n - bf - 1);
+    const uint32_t usable = (uint32_t)(n - cs.bf - 1);
+    const size_t nl = cs.lookups.size();
     cudaStream_t st = ctx->stream;
     DevPool &pool = s->pool;
-    const size_t nl = cs.lookups.size();
-    const Fr one = Fr::one();
-
-    // ---------------------------------------------------------------- theta; mv-lookup prepare (compress, multiplicities)
-    StageTrace trace(st);
-    const Fr theta = tr_squeeze(s);
-    // value-domain column table: [fixed | advice | instance | sigma | omega_pows]
-    const SlotMap vsm{0, cs.nf, cs.nf + cs.na};
-    const uint32_t v_sigma0 = cs.nf + cs.na + cs.ni, v_omega = v_sigma0 + (uint32_t)cs.perm.size();
+    ps.theta = tr_squeeze(s);
+    const SlotMap sm(cs);
     std::vector<Fr *> vcols;
     for (auto p : pk->fixed_values) vcols.push_back(p);
     for (auto p : s->adv_values) vcols.push_back(p);
     for (auto p : s->inst_values) vcols.push_back(p);
     for (auto p : pk->sigma_values) vcols.push_back(p);
     vcols.push_back(pk->omega_pows);
-    Fr **d_vcols = nullptr;
-    ZKB_TRY(upload_table(pool, vcols, &d_vcols, st));
+    ZKB_TRY(upload_table(pool, vcols, &ps.d_vcols, st));
 
-    std::vector<std::vector<Fr *>> lk_f(nl);   // compressed inputs per lookup / input set
-    std::vector<Fr *> lk_t(nl), lk_m(nl);
-    // multi-GPU: lookup argument l is prepared by rank l mod P; m columns live in one slab (+ one word carrying error counts)
-    const Deal lk_deal(ctx, nl);
-    const bool lk_dealt = lk_deal.on;
+    ps.lk_f.resize(nl);
+    ps.lk_t.resize(nl);
+    const Deal deal(ctx, nl);
     Fr *m_slab = nullptr;
-    if (nl) {
-        ZKB_TRY(pool.fr(lk_deal.padded() * n, &m_slab));
-        for (size_t l = 0; l < nl; ++l) lk_m[l] = m_slab + l * n;
-    }
+    ZKB_TRY(dealt_columns(pool, deal, n, ps.lk_m, &m_slab));
     uint64_t lookup_errors = 0;
     for (size_t l = 0; l < nl; ++l) {
-        if (!lk_deal.mine(l)) continue;
+        if (!deal.mine(l)) continue;
         const CsfLookup &lk = cs.lookups[l];
         ExprBuilder eb;
-        ProgramBuilder pb(eb);
         std::vector<int64_t> memo(cs.nodes.size(), -1);
-        std::vector<ProgramBuilder::Root> roots;
-        std::vector<Fr *> outs;
+        std::vector<uint32_t> roots;
         for (size_t j = 0; j < lk.inputs.size(); ++j) {
             Fr *a;
             ZKB_TRY(pool.fr(n, &a));
-            lk_f[l].push_back(a);
-            outs.push_back(a);
-            roots.push_back({compress_exprs(cs, lk.inputs[j], eb, vsm, s->challenges, memo, theta), ProgramBuilder::STORE, (uint32_t)j});
+            ps.lk_f[l].push_back(a);
+            roots.push_back(compress_exprs(cs, lk.inputs[j], eb, sm, s->challenges, memo, ps.theta));
         }
-        ZKB_TRY(pool.fr(n, &lk_t[l]));
-        outs.push_back(lk_t[l]);
-        roots.push_back({compress_exprs(cs, lk.table, eb, vsm, s->challenges, memo, theta), ProgramBuilder::STORE, (uint32_t)lk.inputs.size()});
-        if (!pb.scope(roots)) { set_error("lookup %zu: %s", l, pb.error.c_str()); return ZKB_ERR_ARG; }
-        DeviceProgram dp;
-        ZKB_TRY(upload_program(pool, pb, eb, dp, st));
-        Fr **d_outs = nullptr;
-        ZKB_TRY(upload_table(pool, outs, &d_outs, st));
-        ZKB_TRY(expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_vcols, dp.consts, d_outs, k, 1, 0, st));
+        ZKB_TRY(pool.fr(n, &ps.lk_t[l]));
+        roots.push_back(compress_exprs(cs, lk.table, eb, sm, s->challenges, memo, ps.theta));
+        std::vector<Fr *> outs = ps.lk_f[l];
+        outs.push_back(ps.lk_t[l]);
+        ZKB_TRY(run_store_program(pk, pool, eb, roots, outs, ps.d_vcols, "lookup " + std::to_string(l), st));
         // multiplicities over the usable rows
         uint32_t tsize = 1;
         while (tsize < 2 * usable) tsize <<= 1;
@@ -1101,21 +1124,21 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
         ZKB_CUDA(cudaMemsetAsync(slots, 0, (size_t)tsize * 4, st));
         ZKB_CUDA(cudaMemsetAsync(counts, 0, (size_t)n * 4 + 16, st));
         const unsigned ub = (usable + 255) / 256;
-        m_insert_kernel<<<ub, 256, 0, st>>>(lk_t[l], usable, slots, tsize - 1);
-        for (size_t j = 0; j < lk.inputs.size(); ++j) m_count_kernel<<<ub, 256, 0, st>>>(lk_f[l][j], lk_t[l], usable, slots, tsize - 1, counts, d_err);
-        counts_to_fr_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(counts, (uint32_t)n, lk_m[l]);
+        m_insert_kernel<<<ub, 256, 0, st>>>(ps.lk_t[l], usable, slots, tsize - 1);
+        for (size_t j = 0; j < lk.inputs.size(); ++j) m_count_kernel<<<ub, 256, 0, st>>>(ps.lk_f[l][j], ps.lk_t[l], usable, slots, tsize - 1, counts, d_err);
+        counts_to_fr_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(counts, (uint32_t)n, ps.lk_m[l]);
         ctx->launches += 2 + lk.inputs.size();
         int herr = 0;
         ZKB_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, st));
         ZKB_CUDA(cudaStreamSynchronize(st));
         if (herr) {
             set_error("lookup %zu: an input row is not in the table (unsatisfied witness)", l);
-            if (!lk_dealt) return ZKB_ERR_ARG;
+            if (!deal.on) return ZKB_ERR_ARG;
             lookup_errors++;   // multi-GPU: every rank must learn about it before anyone leaves the collective sequence
         }
     }
-    if (lk_dealt) {
-        ZKB_TRY(deal_gather(ctx, lk_deal, m_slab, n * sizeof(Fr), st));
+    if (deal.on) {
+        ZKB_TRY(deal_gather(ctx, deal, m_slab, n * sizeof(Fr), st));
         uint64_t *d_errw = nullptr;   // every rank learns about an unsatisfied lookup before anyone leaves the collective sequence
         ZKB_TRY(scratch_get(ctx, SCR_COMM_FLAG, 64, (void **)&d_errw));
         ZKB_CUDA(cudaMemcpyAsync(d_errw + 1, &lookup_errors, 8, cudaMemcpyHostToDevice, st));
@@ -1128,218 +1151,230 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
             return ZKB_ERR_ARG;
         }
     }
-    {
-        std::vector<G1Affine> cms;
-        ZKB_TRY(commit_many(pk, lk_m, pk->g_lagrange, n, cms, st));
-        for (auto &cm : cms) ZKB_TRY(tr_write_point(s, cm));
-    }
+    return commit_write(s, ps.lk_m, BASIS_LAGRANGE, st);
+}
 
-    trace.mark("lookups: compress + m + commit");
-    // ---------------------------------------------------------------- beta, gamma; permutation grand products
-    const Fr beta = tr_squeeze(s);
-    const Fr gamma = tr_squeeze(s);
-    auto perm_slot_values = [&](const std::array<uint32_t, 2> &c) -> uint32_t {
-        return c[0] == N_FIXED ? vsm.fixed0 + c[1] : c[0] == N_ADVICE ? vsm.advice0 + c[1] : vsm.instance0 + c[1];
-    };
-    std::vector<Fr *> zs(pk->nsets);
-    {
-        Fr delta;
-        {   // DELTA = 7^(2^28)
-            Fr seven = fr_from_u64(7);
-            delta = seven;
-            for (int i = 0; i < 28; ++i) delta = fp_sqr(delta);
+// permutation/prover.rs commit: beta, gamma, the grand product z of every set of `chunk` permutation columns, z commitments
+static int32_t permutation_commit(zkb_session *s, ProofState &ps, const uint64_t *z_blinds) {
+    zkb_pk *pk = s->pk;
+    zkb_ctx *ctx = pk->ctx;
+    const Csf &cs = pk->cs;
+    const uint64_t n = pk->n;
+    const uint32_t bf = cs.bf;
+    const Fr one = Fr::one();
+    cudaStream_t st = ctx->stream;
+    DevPool &pool = s->pool;
+    ps.beta = tr_squeeze(s);
+    ps.gamma = tr_squeeze(s);
+    const SlotMap sm(cs);
+    const uint32_t v_omega = sm.sigma0 + (uint32_t)cs.perm.size();
+    const Fr delta = perm_delta();
+    // Multi-GPU: the sets are dealt.  Upstream chains them (z_i[0] = last value of z_{i-1}), which is sequential; here every set is
+    // scanned from 1 and rescaled afterwards by c_i = product of the previous sets' last values -- the same field elements
+    // (z_i = c_i * z'_i row by row), with only the nsets last values crossing the ranks before the columns are gathered.
+    const Deal deal(ctx, pk->nsets);
+    Fr *z_slab = nullptr;
+    ZKB_TRY(pool.fr(std::max<size_t>(1, deal.padded()) * n, &z_slab));
+    ps.zs.resize(pk->nsets);
+    for (uint32_t si = 0; si < pk->nsets; ++si) ps.zs[si] = z_slab + (size_t)si * n;
+    Fr *num, *den, *tmp;
+    ZKB_TRY(pool.fr(n, &num));
+    ZKB_TRY(pool.fr(n, &den));
+    ZKB_TRY(pool.fr(n, &tmp));
+    std::vector<Fr> lasts(std::max<size_t>(1, deal.padded()), one);
+    Fr last_z = one;
+    for (uint32_t si = 0; si < pk->nsets; ++si) {
+        if (!deal.mine(si)) continue;
+        ExprBuilder eb;
+        uint32_t nnum = 0, nden = 0;
+        bool first = true;
+        Fr delta_pow = fp_pow_u64(delta, (uint64_t)si * pk->chunk);
+        for (uint32_t j = si * pk->chunk; j < std::min<size_t>((si + 1) * pk->chunk, cs.perm.size()); ++j) {
+            const uint32_t v = eb.col(sm.perm(cs.perm[j]), 0);
+            const uint32_t dterm = eb.add(eb.add(v, eb.mul(eb.col(sm.sigma0 + j, 0), eb.constant(ps.beta))), eb.constant(ps.gamma));
+            const uint32_t nterm = eb.add(eb.add(v, eb.mul(eb.col(v_omega, 0), eb.constant(fp_mul(ps.beta, delta_pow)))), eb.constant(ps.gamma));
+            nden = first ? dterm : eb.mul(nden, dterm);
+            nnum = first ? nterm : eb.mul(nnum, nterm);
+            first = false;
+            delta_pow = fp_mul(delta_pow, delta);
         }
-        // Multi-GPU: the sets are dealt.  Upstream chains them (z_i[0] = last value of z_{i-1}), which is sequential; here every set is
-        // scanned from 1 and rescaled afterwards by c_i = product of the previous sets' last values -- the same field elements
-        // (z_i = c_i * z'_i row by row), with only the nsets last values crossing the ranks before the columns are gathered.
-        const Deal dp_sets(ctx, pk->nsets);
-        Fr *z_slab = nullptr;
-        ZKB_TRY(pool.fr(std::max<size_t>(1, dp_sets.padded()) * n, &z_slab));
-        for (uint32_t si = 0; si < pk->nsets; ++si) zs[si] = z_slab + (size_t)si * n;
-        Fr *num, *den, *tmp;
-        ZKB_TRY(pool.fr(n, &num));
-        ZKB_TRY(pool.fr(n, &den));
-        ZKB_TRY(pool.fr(n, &tmp));
-        std::vector<Fr> lasts(std::max<size_t>(1, dp_sets.padded()), one);
-        Fr last_z = one;
+        ZKB_TRY(run_store_program(pk, pool, eb, {nnum, nden}, {num, den}, ps.d_vcols, "permutation", st));
+        ZKB_TRY(batch_invert_device(ctx, den, tmp, n, st));
+        mul_arrays_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(num, tmp, den, n);  // den <- modified values
+        ctx->launches++;
+        // one GPU: chained exactly like upstream (init = previous last value); dealt: from 1, rescaled below
+        ZKB_TRY(prefix_product_device(ctx, den, n, deal.on ? one : last_z, ps.zs[si], st));
+        ZKB_CUDA(cudaMemcpyAsync(&last_z, ps.zs[si] + (n - bf - 1), sizeof(Fr), cudaMemcpyDeviceToHost, st));
+        ZKB_CUDA(cudaStreamSynchronize(st));
+        lasts[si] = last_z;
+        if (!deal.on) ZKB_CUDA(cudaMemcpyAsync(ps.zs[si] + (n - bf), z_blinds + 4ull * bf * si, (size_t)bf * sizeof(Fr), cudaMemcpyHostToDevice, st));
+    }
+    if (deal.on) {
+        Fr *d_l = nullptr;
+        ZKB_TRY(scratch_get(ctx, SCR_COMM, deal.padded() * sizeof(Fr), (void **)&d_l));
+        ZKB_CUDA(cudaMemcpyAsync(d_l, lasts.data(), deal.padded() * sizeof(Fr), cudaMemcpyHostToDevice, st));
+        ZKB_TRY(deal_gather(ctx, deal, d_l, sizeof(Fr), st));
+        ZKB_CUDA(cudaMemcpyAsync(lasts.data(), d_l, deal.padded() * sizeof(Fr), cudaMemcpyDeviceToHost, st));
+        ZKB_CUDA(cudaStreamSynchronize(st));
+        Fr c = one;   // c_i = prod_{j < i} last'_j
         for (uint32_t si = 0; si < pk->nsets; ++si) {
-            if (!dp_sets.mine(si)) continue;
-            ExprBuilder eb;
-            ProgramBuilder pb(eb);
-            uint32_t nnum = 0, nden = 0;
-            bool first = true;
-            Fr delta_pow = fp_pow_u64(delta, (uint64_t)si * pk->chunk);
-            for (uint32_t j = si * pk->chunk; j < std::min<size_t>((si + 1) * pk->chunk, cs.perm.size()); ++j) {
-                const uint32_t v = eb.col(perm_slot_values(cs.perm[j]), 0);
-                const uint32_t dterm = eb.add(eb.add(v, eb.mul(eb.col(v_sigma0 + j, 0), eb.constant(beta))), eb.constant(gamma));
-                const uint32_t nterm = eb.add(eb.add(v, eb.mul(eb.col(v_omega, 0), eb.constant(fp_mul(beta, delta_pow)))), eb.constant(gamma));
-                nden = first ? dterm : eb.mul(nden, dterm);
-                nnum = first ? nterm : eb.mul(nnum, nterm);
-                first = false;
-                delta_pow = fp_mul(delta_pow, delta);
+            if (deal.mine(si)) {
+                if (!(c == one)) { scale_const_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(ps.zs[si], c, n); ctx->launches++; }
+                ZKB_CUDA(cudaMemcpyAsync(ps.zs[si] + (n - bf), z_blinds + 4ull * bf * si, (size_t)bf * sizeof(Fr), cudaMemcpyHostToDevice, st));
             }
-            if (!pb.scope({{nnum, ProgramBuilder::STORE, 0}, {nden, ProgramBuilder::STORE, 1}})) { set_error("permutation: %s", pb.error.c_str()); return ZKB_ERR_ARG; }
-            DeviceProgram dp;
-            ZKB_TRY(upload_program(pool, pb, eb, dp, st));
-            std::vector<Fr *> outs{num, den};
-            Fr **d_outs = nullptr;
-            ZKB_TRY(upload_table(pool, outs, &d_outs, st));
-            ZKB_TRY(expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_vcols, dp.consts, d_outs, k, 1, 0, st));
-            ZKB_TRY(batch_invert_device(ctx, den, tmp, n, st));
-            mul_arrays_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(num, tmp, den, n);  // den <- modified values
-            ctx->launches++;
-            // one GPU: chained exactly like upstream (init = previous last value); dealt: from 1, rescaled below
-            ZKB_TRY(prefix_product_device(ctx, den, n, dp_sets.on ? one : last_z, zs[si], st));
-            ZKB_CUDA(cudaMemcpyAsync(&last_z, zs[si] + (n - bf - 1), sizeof(Fr), cudaMemcpyDeviceToHost, st));
-            ZKB_CUDA(cudaStreamSynchronize(st));
-            lasts[si] = last_z;
-            if (!dp_sets.on) ZKB_CUDA(cudaMemcpyAsync(zs[si] + (n - bf), z_blinds + 4ull * bf * si, (size_t)bf * sizeof(Fr), cudaMemcpyHostToDevice, st));
+            c = fp_mul(c, lasts[si]);
         }
-        if (dp_sets.on) {
-            Fr *d_l = nullptr;
-            ZKB_TRY(scratch_get(ctx, SCR_COMM, dp_sets.padded() * sizeof(Fr), (void **)&d_l));
-            ZKB_CUDA(cudaMemcpyAsync(d_l, lasts.data(), dp_sets.padded() * sizeof(Fr), cudaMemcpyHostToDevice, st));
-            ZKB_TRY(deal_gather(ctx, dp_sets, d_l, sizeof(Fr), st));
-            ZKB_CUDA(cudaMemcpyAsync(lasts.data(), d_l, dp_sets.padded() * sizeof(Fr), cudaMemcpyDeviceToHost, st));
-            ZKB_CUDA(cudaStreamSynchronize(st));
-            Fr c = one;   // c_i = prod_{j < i} last'_j
-            for (uint32_t si = 0; si < pk->nsets; ++si) {
-                if (dp_sets.mine(si)) {
-                    if (!(c == one)) { scale_const_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(zs[si], c, n); ctx->launches++; }
-                    ZKB_CUDA(cudaMemcpyAsync(zs[si] + (n - bf), z_blinds + 4ull * bf * si, (size_t)bf * sizeof(Fr), cudaMemcpyHostToDevice, st));
-                }
-                c = fp_mul(c, lasts[si]);
-            }
-            ZKB_TRY(deal_gather(ctx, dp_sets, z_slab, n * sizeof(Fr), st));
-        }
+        ZKB_TRY(deal_gather(ctx, deal, z_slab, n * sizeof(Fr), st));
     }
-    {
-        std::vector<G1Affine> cms;
-        ZKB_TRY(commit_many(pk, zs, pk->g_lagrange, n, cms, st));
-        for (auto &cm : cms) ZKB_TRY(tr_write_point(s, cm));
-    }
+    return commit_write(s, ps.zs, BASIS_LAGRANGE, st);
+}
 
-    trace.mark("permutation z + commit");
-    // ---------------------------------------------------------------- lookup grand sums phi
-    std::vector<Fr *> phis(nl);
+// mv_lookup/prover.rs commit_grand_sum: phi = prefix sums of sum_j 1/(f_j + beta) - m/(t + beta), all denominators of a lookup
+// inverted at once; phi commitments.  Multi-GPU: dealt like the multiplicities.
+static int32_t lookup_commit_grand_sum(zkb_session *s, ProofState &ps, const uint64_t *phi_blinds) {
+    zkb_pk *pk = s->pk;
+    zkb_ctx *ctx = pk->ctx;
+    const uint64_t n = pk->n;
+    const uint32_t bf = pk->cs.bf;
+    const size_t nl = pk->cs.lookups.size();
+    cudaStream_t st = ctx->stream;
+    DevPool &pool = s->pool;
+    const Deal deal(ctx, nl);
     Fr *phi_slab = nullptr;
-    if (nl) {
-        ZKB_TRY(pool.fr(lk_deal.padded() * n, &phi_slab));
-        for (size_t l = 0; l < nl; ++l) phis[l] = phi_slab + l * n;
-    }
+    ZKB_TRY(dealt_columns(pool, deal, n, ps.phis, &phi_slab));
     for (size_t l = 0; l < nl; ++l) {
-        if (!lk_deal.mine(l)) continue;
-        const size_t J = lk_f[l].size();
+        if (!deal.mine(l)) continue;
+        const size_t J = ps.lk_f[l].size();
         // denominators (f_j + beta), (t + beta) into one contiguous array, inverted at once
         Fr *dens, *invs, *dterm;
         ZKB_TRY(pool.fr((J + 1) * n, &dens));
         ZKB_TRY(pool.fr((J + 1) * n, &invs));
         ZKB_TRY(pool.fr(n, &dterm));
-        std::vector<Fr *> cols;
-        for (auto p : lk_f[l]) cols.push_back(p);
-        cols.push_back(lk_t[l]);          // slot J
-        cols.push_back(lk_m[l]);          // slot J + 1
+        std::vector<Fr *> cols = ps.lk_f[l];
+        cols.push_back(ps.lk_t[l]);       // slot J
+        cols.push_back(ps.lk_m[l]);       // slot J + 1
         for (size_t j = 0; j <= J; ++j) cols.push_back(invs + j * n);  // slots J + 2 ..
         Fr **d_cols = nullptr;
         ZKB_TRY(upload_table(pool, cols, &d_cols, st));
         {
             ExprBuilder eb;
-            ProgramBuilder pb(eb);
-            std::vector<ProgramBuilder::Root> roots;
+            std::vector<uint32_t> roots;
             std::vector<Fr *> outs;
             for (size_t j = 0; j <= J; ++j) {
-                roots.push_back({eb.add(eb.col((uint32_t)j, 0), eb.constant(beta)), ProgramBuilder::STORE, (uint32_t)j});
+                roots.push_back(eb.add(eb.col((uint32_t)j, 0), eb.constant(ps.beta)));
                 outs.push_back(dens + j * n);
             }
-            if (!pb.scope(roots)) { set_error("lookup sum: %s", pb.error.c_str()); return ZKB_ERR_ARG; }
-            DeviceProgram dp;
-            ZKB_TRY(upload_program(pool, pb, eb, dp, st));
-            Fr **d_outs = nullptr;
-            ZKB_TRY(upload_table(pool, outs, &d_outs, st));
-            ZKB_TRY(expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, k, 1, 0, st));
+            ZKB_TRY(run_store_program(pk, pool, eb, roots, outs, d_cols, "lookup sum", st));
         }
         ZKB_TRY(batch_invert_device(ctx, dens, invs, (J + 1) * n, st));
         {
             ExprBuilder eb;
-            ProgramBuilder pb(eb);
             uint32_t acc = eb.neg(eb.mul(eb.col((uint32_t)J + 1, 0), eb.col((uint32_t)(J + 2 + J), 0)));  // - m / (t + beta)
             for (size_t j = 0; j < J; ++j) acc = eb.add(acc, eb.col((uint32_t)(J + 2 + j), 0));
-            if (!pb.scope({{acc, ProgramBuilder::STORE, 0}})) { set_error("lookup sum: %s", pb.error.c_str()); return ZKB_ERR_ARG; }
-            DeviceProgram dp;
-            ZKB_TRY(upload_program(pool, pb, eb, dp, st));
-            std::vector<Fr *> outs{dterm};
-            Fr **d_outs = nullptr;
-            ZKB_TRY(upload_table(pool, outs, &d_outs, st));
-            ZKB_TRY(expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, k, 1, 0, st));
+            ZKB_TRY(run_store_program(pk, pool, eb, {acc}, {dterm}, d_cols, "lookup sum", st));
         }
-        ZKB_TRY(prefix_sum_device(ctx, dterm, n, Fr::zero(), phis[l], st));
-        ZKB_CUDA(cudaMemcpyAsync(phis[l] + (n - bf), phi_blinds + 4ull * bf * l, (size_t)bf * sizeof(Fr), cudaMemcpyHostToDevice, st));
+        ZKB_TRY(prefix_sum_device(ctx, dterm, n, Fr::zero(), ps.phis[l], st));
+        ZKB_CUDA(cudaMemcpyAsync(ps.phis[l] + (n - bf), phi_blinds + 4ull * bf * l, (size_t)bf * sizeof(Fr), cudaMemcpyHostToDevice, st));
     }
-    if (nl) ZKB_TRY(deal_gather(ctx, lk_deal, phi_slab, n * sizeof(Fr), st));
-    {
-        std::vector<G1Affine> cms;
-        ZKB_TRY(commit_many(pk, phis, pk->g_lagrange, n, cms, st));
-        for (auto &cm : cms) ZKB_TRY(tr_write_point(s, cm));
-    }
+    if (nl) ZKB_TRY(deal_gather(ctx, deal, phi_slab, n * sizeof(Fr), st));
+    return commit_write(s, ps.phis, BASIS_LAGRANGE, st);
+}
 
-    trace.mark("lookup phi + commit");
-    // ---------------------------------------------------------------- vanishing: random polynomial
-    Fr *random_poly;
-    ZKB_TRY(pool.fr(n, &random_poly));
-    ZKB_CUDA(cudaMemcpyAsync(random_poly, random_poly_host, n * sizeof(Fr), cudaMemcpyHostToDevice, st));
-    {
-        G1Affine cm;
-        { std::vector<Fr *> one_col{random_poly}; std::vector<G1Affine> r1; ZKB_TRY(commit_many(pk, one_col, pk->g, n, r1, st)); cm = r1[0]; }
-        ZKB_TRY(tr_write_point(s, cm));
-    }
-    const Fr y = tr_squeeze(s);
+// vanishing/prover.rs commit: the caller's random polynomial (coefficients) committed against g, then y
+static int32_t vanishing_commit(zkb_session *s, ProofState &ps, const uint64_t *random_poly_host) {
+    zkb_pk *pk = s->pk;
+    cudaStream_t st = pk->ctx->stream;
+    ZKB_TRY(s->pool.fr(pk->n, &ps.random_poly));
+    ZKB_CUDA(cudaMemcpyAsync(ps.random_poly, random_poly_host, pk->n * sizeof(Fr), cudaMemcpyHostToDevice, st));
+    ZKB_TRY(commit_write(s, {ps.random_poly}, BASIS_G, st));
+    ps.y = tr_squeeze(s);
+    return ZKB_OK;
+}
 
-    trace.mark("random poly commit");
-    // ---------------------------------------------------------------- coefficient forms
-    const uint32_t ntt_chunk = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(256, (1ull << 31) / (n * sizeof(Fr))));  // <= 2 GiB of NTT scratch
-    auto ntt_many = [&](const std::vector<Fr *> &src, const std::vector<Fr *> &dst, const Fr &w, const Fr *scale, const Fr *in_scale) -> int32_t {
-        for (size_t done = 0; done < src.size(); done += ntt_chunk) {
-            const uint32_t cur = (uint32_t)std::min<size_t>(ntt_chunk, src.size() - done);
-            std::vector<Fr *> a(src.begin() + done, src.begin() + done + cur), b(dst.begin() + done, dst.begin() + done + cur);
-            ZKB_TRY(ntt_fr_batch_device(ctx, a.data(), b.data(), cur, k, w, scale, 0, in_scale, st));
+// Lagrange -> coefficient form of `vals` into a new slab.  Multi-GPU: contiguous blocks of columns per rank, one all-gather.
+static int32_t to_coeff_dealt(zkb_session *s, const std::vector<Fr *> &vals, std::vector<Fr *> &polys) {
+    zkb_pk *pk = s->pk;
+    const Deal dc(pk->ctx, vals.size());
+    Fr *pslab = nullptr;
+    ZKB_TRY(dealt_columns(s->pool, dc, pk->n, polys, &pslab));
+    if (vals.empty()) return ZKB_OK;
+    std::vector<Fr *> src, dst;
+    for (size_t i = 0; i < vals.size(); ++i)
+        if (dc.mine(i)) { src.push_back(vals[i]); dst.push_back(polys[i]); }
+    if (!src.empty()) ZKB_TRY(ntt_many(pk, src, dst, pk->omega_inv, &pk->n_inv, nullptr, pk->ctx->stream));
+    return deal_gather(pk->ctx, dc, pslab, pk->n * sizeof(Fr), pk->ctx->stream);
+}
+static int32_t coefficient_forms(zkb_session *s, ProofState &ps) {
+    ZKB_TRY(to_coeff_dealt(s, s->adv_values, ps.adv_polys));
+    ZKB_TRY(to_coeff_dealt(s, ps.zs, ps.z_polys));
+    ZKB_TRY(to_coeff_dealt(s, ps.phis, ps.phi_polys));
+    return to_coeff_dealt(s, ps.lk_m, ps.m_polys);
+}
+
+// Gate polynomials of the quotient program, Horner in y in constraint-system order.  Circuits multiply whole groups of constraints
+// by one selector (`q_enable * constraint`), so runs of CONSECUTIVE gates of the form fixed(col, rot) * t_j are folded exactly:
+//   (..(acc y + f t_1) y + ..) y + f t_r  =  acc y^r + f (t_1 y^(r-1) + .. + t_r)
+// -- the same field element (distributivity is exact mod r), one multiply per gate less than the term-by-term form.
+static int32_t quotient_gates(const Csf &cs, const std::vector<Fr> &challenges, ExprBuilder &qeb, ProgramBuilder &qpb, const SlotMap &sm,
+                              std::vector<int64_t> &memo, const Fr &y, uint32_t y_idx) {
+    auto selector_split = [&](uint32_t gnode, uint32_t &sel, uint32_t &rest) -> bool {
+        const auto &nd = cs.nodes[gnode];
+        if (nd[0] != N_MUL) return false;
+        for (int side = 0; side < 2; ++side) {
+            const uint32_t a = nd[1 + side], b = nd[2 - side];
+            if (cs.nodes[a][0] == N_FIXED) { sel = a; rest = b; return true; }
         }
-        return ZKB_OK;
+        return false;
     };
-    auto to_coeff_new = [&](const std::vector<Fr *> &vals, std::vector<Fr *> &polys) -> int32_t {
-        polys.resize(vals.size());
-        if (vals.empty()) return ZKB_OK;
-        Fr *pslab = nullptr;
-        const Deal dc(ctx, vals.size());   // multi-GPU: contiguous blocks of columns per rank, completed by one all-gather
-        ZKB_TRY(pool.fr(dc.padded() * n, &pslab));
-        for (size_t i = 0; i < vals.size(); ++i) polys[i] = pslab + i * n;
-        std::vector<Fr *> src, dst;
-        for (size_t i = 0; i < vals.size(); ++i)
-            if (dc.mine(i)) { src.push_back(vals[i]); dst.push_back(polys[i]); }
-        if (!src.empty()) ZKB_TRY(ntt_many(src, dst, pk->omega_inv, &pk->n_inv, nullptr));
-        ZKB_TRY(deal_gather(ctx, dc, pslab, n * sizeof(Fr), st));
-        return ZKB_OK;
-    };
-    std::vector<Fr *> adv_polys, z_polys, phi_polys, m_polys;
-    ZKB_TRY(to_coeff_new(s->adv_values, adv_polys));
-    ZKB_TRY(to_coeff_new(zs, z_polys));
-    ZKB_TRY(to_coeff_new(phis, phi_polys));
-    ZKB_TRY(to_coeff_new(lk_m, m_polys));
+    auto same_query = [&](uint32_t a, uint32_t b) { return cs.nodes[a][1] == cs.nodes[b][1] && cs.nodes[a][2] == cs.nodes[b][2]; };
+    for (size_t gi = 0; gi < cs.gates.size();) {
+        uint32_t sel = 0, rest = 0;
+        size_t run = 1;
+        if (selector_split(cs.gates[gi], sel, rest)) {
+            uint32_t s2 = 0, r2 = 0;
+            while (gi + run < cs.gates.size() && run < 4096 && selector_split(cs.gates[gi + run], s2, r2) && same_query(sel, s2)) ++run;
+        }
+        if (run < 2) {
+            if (!qpb.scope({{translate(cs, cs.gates[gi], qeb, sm, challenges, memo), ProgramBuilder::HORNER, y_idx}})) { set_error("gate: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
+            ++gi;
+            continue;
+        }
+        for (size_t t = 0; t < run; ++t) {
+            uint32_t s2 = 0, r2 = 0;
+            selector_split(cs.gates[gi + t], s2, r2);
+            if (!qpb.scope({{translate(cs, r2, qeb, sm, challenges, memo), ProgramBuilder::HORNER2, y_idx}})) { set_error("gate: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
+        }
+        const uint32_t yr_idx = qeb.const_slot(fp_pow_u64(y, run));
+        if (!qpb.scope({{translate(cs, sel, qeb, sm, challenges, memo), ProgramBuilder::FOLD, yr_idx}})) { set_error("gate: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
+        gi += run;
+    }
+    return ZKB_OK;
+}
 
-    trace.mark("lagrange_to_coeff (all columns)");
-    // ---------------------------------------------------------------- quotient numerator program (plonk/evaluation.rs order)
+// evaluation.rs evaluate_h: the quotient numerator program (gates, permutation, lookups, in upstream's y-Horner order), then
+// per coset part j the coset NTTs of every polynomial not in the pk's coset cache and ONE interpreter launch, x 1/((zeta w^j)^n - 1)
+static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
+    zkb_pk *pk = s->pk;
+    zkb_ctx *ctx = pk->ctx;
+    const Csf &cs = pk->cs;
+    const uint64_t n = pk->n;
+    const uint32_t k = cs.k;
+    const Fr one = Fr::one();
+    cudaStream_t st = ctx->stream;
+    DevPool &pool = s->pool;
     // coset-domain slot table: [fixed | advice | instance | sigma | z | phi | m | l0 | l_last | l_blind | X]
+    const SlotMap sm(cs);
     std::vector<Fr *> qpolys;
     for (auto p : pk->fixed_polys) qpolys.push_back(p);
-    for (auto p : adv_polys) qpolys.push_back(p);
+    for (auto p : ps.adv_polys) qpolys.push_back(p);
     for (auto p : s->inst_polys) qpolys.push_back(p);
-    const uint32_t q_sigma0 = (uint32_t)qpolys.size();
     for (auto p : pk->sigma_polys) qpolys.push_back(p);
     const uint32_t q_z0 = (uint32_t)qpolys.size();
-    for (auto p : z_polys) qpolys.push_back(p);
+    for (auto p : ps.z_polys) qpolys.push_back(p);
     const uint32_t q_phi0 = (uint32_t)qpolys.size();
-    for (auto p : phi_polys) qpolys.push_back(p);
+    for (auto p : ps.phi_polys) qpolys.push_back(p);
     const uint32_t q_m0 = (uint32_t)qpolys.size();
-    for (auto p : m_polys) qpolys.push_back(p);
+    for (auto p : ps.m_polys) qpolys.push_back(p);
     const uint32_t q_l0 = (uint32_t)qpolys.size();
     qpolys.push_back(pk->l0_poly);
     qpolys.push_back(pk->llast_poly);
@@ -1347,133 +1382,87 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
     qpolys.push_back(pk->xid_poly);
     const uint32_t q_llast = q_l0 + 1, q_lblind = q_l0 + 2, q_x = q_l0 + 3;
     ZKB_ARG(qpolys.size() < 65536);
-    const SlotMap qsm{0, cs.nf, cs.nf + cs.na};
 
     ExprBuilder qeb;
     ProgramBuilder qpb(qeb);
-    const uint32_t y_idx = qeb.const_slot(y);
-    {
-        std::vector<int64_t> memo(cs.nodes.size(), -1);
-        // Gate polynomials, Horner in y in constraint-system order.  Circuits multiply whole groups of constraints by one selector
-        // (`q_enable * constraint`), so runs of CONSECUTIVE gates of the form fixed(col, rot) * t_j are folded exactly:
-        //   (..(acc y + f t_1) y + ..) y + f t_r  =  acc y^r + f (t_1 y^(r-1) + .. + t_r)
-        // -- the same field element (distributivity is exact mod r), one multiply per gate less than the term-by-term form.
-        auto selector_split = [&](uint32_t gnode, uint32_t &sel, uint32_t &rest) -> bool {
-            const auto &nd = cs.nodes[gnode];
-            if (nd[0] != N_MUL) return false;
-            for (int side = 0; side < 2; ++side) {
-                const uint32_t a = nd[1 + side], b = nd[2 - side];
-                if (cs.nodes[a][0] == N_FIXED) { sel = a; rest = b; return true; }
-            }
-            return false;
-        };
-        auto same_query = [&](uint32_t a, uint32_t b) { return cs.nodes[a][1] == cs.nodes[b][1] && cs.nodes[a][2] == cs.nodes[b][2]; };
-        const bool fold_runs = !(getenv("ZKB_NO_SELECTOR_FOLD") && getenv("ZKB_NO_SELECTOR_FOLD")[0] == '1');
-        for (size_t gi = 0; gi < cs.gates.size();) {
-            uint32_t sel = 0, rest = 0;
-            size_t run = 1;
-            if (fold_runs && selector_split(cs.gates[gi], sel, rest)) {
-                uint32_t s2 = 0, r2 = 0;
-                while (gi + run < cs.gates.size() && run < 4096 && selector_split(cs.gates[gi + run], s2, r2) && same_query(sel, s2)) ++run;
-            }
-            if (run < 2) {
-                if (!qpb.scope({{translate(cs, cs.gates[gi], qeb, qsm, s->challenges, memo), ProgramBuilder::HORNER, y_idx}})) { set_error("gate: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
-                ++gi;
-                continue;
-            }
-            for (size_t t = 0; t < run; ++t) {
-                uint32_t s2 = 0, r2 = 0;
-                selector_split(cs.gates[gi + t], s2, r2);
-                if (!qpb.scope({{translate(cs, r2, qeb, qsm, s->challenges, memo), ProgramBuilder::HORNER2, y_idx}})) { set_error("gate: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
-            }
-            const uint32_t yr_idx = qeb.const_slot(fp_pow_u64(y, run));
-            if (!qpb.scope({{translate(cs, sel, qeb, qsm, s->challenges, memo), ProgramBuilder::FOLD, yr_idx}})) { set_error("gate: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
-            gi += run;
+    const uint32_t y_idx = qeb.const_slot(ps.y);
+    std::vector<int64_t> memo(cs.nodes.size(), -1);
+    ZKB_TRY(quotient_gates(cs, s->challenges, qeb, qpb, sm, memo, ps.y, y_idx));
+    auto lactive = [&]() { return qeb.sub(qeb.sub(qeb.constant(one), qeb.col(q_llast, 0)), qeb.col(q_lblind, 0)); };
+    if (pk->nsets) {
+        const uint32_t z0 = qeb.col(q_z0, 0), zl = qeb.col(q_z0 + pk->nsets - 1, 0);
+        if (!qpb.scope({{qeb.mul(qeb.sub(qeb.constant(one), z0), qeb.col(q_l0, 0)), ProgramBuilder::HORNER, y_idx}})) return ZKB_ERR_ARG;
+        if (!qpb.scope({{qeb.mul(qeb.sub(qeb.mul(zl, zl), zl), qeb.col(q_llast, 0)), ProgramBuilder::HORNER, y_idx}})) return ZKB_ERR_ARG;
+        for (uint32_t i = 1; i < pk->nsets; ++i) {
+            const uint32_t t = qeb.mul(qeb.sub(qeb.col(q_z0 + i, 0), qeb.col(q_z0 + i - 1, -(int32_t)(cs.bf + 1))), qeb.col(q_l0, 0));
+            if (!qpb.scope({{t, ProgramBuilder::HORNER, y_idx}})) return ZKB_ERR_ARG;
         }
-        auto lactive = [&]() { return qeb.sub(qeb.sub(qeb.constant(one), qeb.col(q_llast, 0)), qeb.col(q_lblind, 0)); };
-        if (pk->nsets) {
-            const uint32_t z0 = qeb.col(q_z0, 0), zl = qeb.col(q_z0 + pk->nsets - 1, 0);
-            if (!qpb.scope({{qeb.mul(qeb.sub(qeb.constant(one), z0), qeb.col(q_l0, 0)), ProgramBuilder::HORNER, y_idx}})) return ZKB_ERR_ARG;
-            if (!qpb.scope({{qeb.mul(qeb.sub(qeb.mul(zl, zl), zl), qeb.col(q_llast, 0)), ProgramBuilder::HORNER, y_idx}})) return ZKB_ERR_ARG;
-            for (uint32_t i = 1; i < pk->nsets; ++i) {
-                const uint32_t t = qeb.mul(qeb.sub(qeb.col(q_z0 + i, 0), qeb.col(q_z0 + i - 1, -(int32_t)(bf + 1))), qeb.col(q_l0, 0));
-                if (!qpb.scope({{t, ProgramBuilder::HORNER, y_idx}})) return ZKB_ERR_ARG;
+        const Fr delta = perm_delta();
+        Fr delta_pow = one;
+        for (uint32_t si = 0; si < pk->nsets; ++si) {
+            uint32_t left = qeb.col(q_z0 + si, 1), right = qeb.col(q_z0 + si, 0);
+            for (uint32_t j = si * pk->chunk; j < std::min<size_t>((si + 1) * pk->chunk, cs.perm.size()); ++j) {
+                const uint32_t v = qeb.col(sm.perm(cs.perm[j]), 0);
+                left = qeb.mul(left, qeb.add(qeb.add(v, qeb.mul(qeb.col(sm.sigma0 + j, 0), qeb.constant(ps.beta))), qeb.constant(ps.gamma)));
+                right = qeb.mul(right, qeb.add(qeb.add(v, qeb.mul(qeb.col(q_x, 0), qeb.constant(fp_mul(ps.beta, delta_pow)))), qeb.constant(ps.gamma)));
+                delta_pow = fp_mul(delta_pow, delta);
             }
-            Fr delta_pow = one, delta;
-            {
-                Fr seven = fr_from_u64(7);
-                delta = seven;
-                for (int i = 0; i < 28; ++i) delta = fp_sqr(delta);
-            }
-            for (uint32_t si = 0; si < pk->nsets; ++si) {
-                uint32_t left = qeb.col(q_z0 + si, 1), right = qeb.col(q_z0 + si, 0);
-                for (uint32_t j = si * pk->chunk; j < std::min<size_t>((si + 1) * pk->chunk, cs.perm.size()); ++j) {
-                    const auto &c = cs.perm[j];
-                    const uint32_t vslot = c[0] == N_FIXED ? qsm.fixed0 + c[1] : c[0] == N_ADVICE ? qsm.advice0 + c[1] : qsm.instance0 + c[1];
-                    const uint32_t v = qeb.col(vslot, 0);
-                    left = qeb.mul(left, qeb.add(qeb.add(v, qeb.mul(qeb.col(q_sigma0 + j, 0), qeb.constant(beta))), qeb.constant(gamma)));
-                    right = qeb.mul(right, qeb.add(qeb.add(v, qeb.mul(qeb.col(q_x, 0), qeb.constant(fp_mul(beta, delta_pow)))), qeb.constant(gamma)));
-                    delta_pow = fp_mul(delta_pow, delta);
-                }
-                if (!qpb.scope({{qeb.mul(qeb.sub(left, right), lactive()), ProgramBuilder::HORNER, y_idx}})) { set_error("permutation: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
-            }
-        }
-        for (size_t l = 0; l < nl; ++l) {
-            const CsfLookup &lk = cs.lookups[l];
-            std::vector<uint32_t> fsb;
-            for (auto &inp : lk.inputs) fsb.push_back(qeb.add(compress_exprs(cs, inp, qeb, qsm, s->challenges, memo, theta), qeb.constant(beta)));
-            const uint32_t tb = qeb.add(compress_exprs(cs, lk.table, qeb, qsm, s->challenges, memo, theta), qeb.constant(beta));
-            uint32_t prod = fsb[0];
-            for (size_t j = 1; j < fsb.size(); ++j) prod = qeb.mul(prod, fsb[j]);
-            uint32_t ssum = 0;
-            bool have_sum = false;
-            for (size_t i = 0; i < fsb.size(); ++i) {
-                uint32_t pr = 0;
-                bool have = false;
-                for (size_t j = 0; j < fsb.size(); ++j) {
-                    if (j == i) continue;
-                    pr = have ? qeb.mul(pr, fsb[j]) : fsb[j];
-                    have = true;
-                }
-                if (!have) pr = qeb.constant(one);
-                ssum = have_sum ? qeb.add(ssum, pr) : pr;
-                have_sum = true;
-            }
-            const uint32_t phi = qeb.col(q_phi0 + (uint32_t)l, 0), phi_next = qeb.col(q_phi0 + (uint32_t)l, 1), m = qeb.col(q_m0 + (uint32_t)l, 0);
-            const uint32_t lhs = qeb.mul(qeb.mul(tb, prod), qeb.sub(phi_next, phi));
-            const uint32_t rhs = qeb.sub(qeb.mul(tb, ssum), qeb.mul(m, prod));
-            std::vector<ProgramBuilder::Root> roots = {{qeb.mul(phi, qeb.col(q_l0, 0)), ProgramBuilder::HORNER, y_idx},
-                                                       {qeb.mul(phi, qeb.col(q_llast, 0)), ProgramBuilder::HORNER, y_idx},
-                                                       {qeb.mul(qeb.sub(lhs, rhs), lactive()), ProgramBuilder::HORNER, y_idx}};
-            if (!qpb.scope(roots)) { set_error("lookup %zu: %s", l, qpb.error.c_str()); return ZKB_ERR_ARG; }
+            if (!qpb.scope({{qeb.mul(qeb.sub(left, right), lactive()), ProgramBuilder::HORNER, y_idx}})) { set_error("permutation: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
         }
     }
-    // one STOREACC per coset part (the scale constant differs): emit them as separate tiny programs appended at launch
+    for (size_t l = 0; l < cs.lookups.size(); ++l) {
+        const CsfLookup &lk = cs.lookups[l];
+        std::vector<uint32_t> fsb;
+        for (auto &inp : lk.inputs) fsb.push_back(qeb.add(compress_exprs(cs, inp, qeb, sm, s->challenges, memo, ps.theta), qeb.constant(ps.beta)));
+        const uint32_t tb = qeb.add(compress_exprs(cs, lk.table, qeb, sm, s->challenges, memo, ps.theta), qeb.constant(ps.beta));
+        uint32_t prod = fsb[0];
+        for (size_t j = 1; j < fsb.size(); ++j) prod = qeb.mul(prod, fsb[j]);
+        uint32_t ssum = 0;
+        bool have_sum = false;
+        for (size_t i = 0; i < fsb.size(); ++i) {
+            uint32_t pr = 0;
+            bool have = false;
+            for (size_t j = 0; j < fsb.size(); ++j) {
+                if (j == i) continue;
+                pr = have ? qeb.mul(pr, fsb[j]) : fsb[j];
+                have = true;
+            }
+            if (!have) pr = qeb.constant(one);
+            ssum = have_sum ? qeb.add(ssum, pr) : pr;
+            have_sum = true;
+        }
+        const uint32_t phi = qeb.col(q_phi0 + (uint32_t)l, 0), phi_next = qeb.col(q_phi0 + (uint32_t)l, 1), m = qeb.col(q_m0 + (uint32_t)l, 0);
+        const uint32_t lhs = qeb.mul(qeb.mul(tb, prod), qeb.sub(phi_next, phi));
+        const uint32_t rhs = qeb.sub(qeb.mul(tb, ssum), qeb.mul(m, prod));
+        std::vector<ProgramBuilder::Root> roots = {{qeb.mul(phi, qeb.col(q_l0, 0)), ProgramBuilder::HORNER, y_idx},
+                                                   {qeb.mul(phi, qeb.col(q_llast, 0)), ProgramBuilder::HORNER, y_idx},
+                                                   {qeb.mul(qeb.sub(lhs, rhs), lactive()), ProgramBuilder::HORNER, y_idx}};
+        if (!qpb.scope(roots)) { set_error("lookup %zu: %s", l, qpb.error.c_str()); return ZKB_ERR_ARG; }
+    }
+    // one STOREACC per coset part (the scale constant differs): the device code buffer holds the common body + one trailing
+    // STOREACC slot that is rewritten per part
     std::vector<uint32_t> tinv_idx(pk->E);
     for (uint32_t j = 0; j < pk->E; ++j) tinv_idx[j] = qeb.const_slot(pk->t_inv[j]);
     const size_t base_len = qpb.code.size();
     DeviceProgram qdp;
-    {
-        // device code buffer holds the common body + one trailing STOREACC slot that is rewritten per part
-        qpb.store_acc(0, tinv_idx[0]);
-        ZKB_TRY(upload_program(pool, qpb, qeb, qdp, st));
-    }
-
+    qpb.store_acc(0, tinv_idx[0]);
+    ZKB_TRY(upload_program(pool, qpb, qeb, qdp, st));
     trace.mark("quotient program build+upload");
-    // ---------------------------------------------------------------- evaluate h on the extended domain, part by part
-    Fr *slab, *pows, *h_ext;
+
+    // evaluate h on the extended domain, part by part
+    Fr *slab, *pows;
     ZKB_TRY(pool.fr(qpolys.size() * n, &slab));
     ZKB_TRY(pool.fr(n, &pows));
-    ZKB_TRY(pool.fr(pk->N, &h_ext));
+    ZKB_TRY(pool.fr(pk->N, &ps.h_ext));
     std::vector<Fr *> qcols(qpolys.size());
     for (size_t i = 0; i < qpolys.size(); ++i) qcols[i] = slab + i * n;
-    // slots served from the pk's coset cache: fixed [0, nf), sigma, l0 / l_last / l_blind / X
+    // slots served from the pk's coset cache: fixed, sigma, l0 / l_last / l_blind / X
     const bool cached = !pk->coset_cache.empty();
     std::vector<int> cache_idx(qpolys.size(), -1);
     if (cached) {
         int ci = 0;
-        for (uint32_t i = 0; i < cs.nf; ++i) cache_idx[qsm.fixed0 + i] = ci++;
-        for (size_t i = 0; i < cs.perm.size(); ++i) cache_idx[q_sigma0 + i] = ci++;
+        for (uint32_t i = 0; i < cs.nf; ++i) cache_idx[sm.fixed0 + i] = ci++;
+        for (size_t i = 0; i < cs.perm.size(); ++i) cache_idx[sm.sigma0 + i] = ci++;
         cache_idx[q_l0] = ci++; cache_idx[q_llast] = ci++; cache_idx[q_lblind] = ci++; cache_idx[q_x] = ci++;
     }
     std::vector<Fr *> ntt_src, ntt_dst;
@@ -1482,7 +1471,7 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
     }
     Fr **d_qcols = nullptr, **d_hout = nullptr;
     ZKB_TRY(pool.alloc(qcols.size() * sizeof(Fr *) + 8, (void **)&d_qcols));
-    std::vector<Fr *> hout{h_ext};
+    std::vector<Fr *> hout{ps.h_ext};
     ZKB_TRY(upload_table(pool, hout, &d_hout, st));
     // multi-GPU: coset parts are dealt in contiguous blocks; a rank writes its parts as contiguous n-element rows of h_parts, the rows
     // are all-gathered and interleaved into the extended-domain order h_ext[j + E i] the inverse transform expects
@@ -1496,9 +1485,8 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
     }
     for (uint32_t j = 0; j < pk->E; ++j) {
         if (!dq.mine(j)) continue;
-        const Fr gj = fp_mul(pk->zeta, fp_pow_u64(pk->ext_omega, j));
-        ZKB_TRY(fr_powers_device(ctx, gj, n, pows, st));
-        ZKB_TRY(ntt_many(ntt_src, ntt_dst, pk->omega, nullptr, pows));
+        ZKB_TRY(fr_powers_device(ctx, pk->coset_gen(j), n, pows, st));
+        ZKB_TRY(ntt_many(pk, ntt_src, ntt_dst, pk->omega, nullptr, pows, st));
         std::vector<Fr *> cols_j = qcols;
         if (cached)
             for (size_t i = 0; i < qpolys.size(); ++i)
@@ -1512,41 +1500,45 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
     }
     if (dq.on) {
         ZKB_TRY(deal_gather(ctx, dq, h_parts, n * sizeof(Fr), st));
-        interleave_parts_kernel<<<(unsigned)((pk->N + 255) / 256), 256, 0, st>>>(h_parts, h_ext, k, pk->E);
+        interleave_parts_kernel<<<(unsigned)((pk->N + 255) / 256), 256, 0, st>>>(h_parts, ps.h_ext, k, pk->E);
         ctx->launches++;
     }
-    trace.mark("quotient: coset NTTs + fused eval");
-    // extended_to_coeff: inverse NTT over the extended domain, 1/N, undo the zeta coset, keep n*(d-1) coefficients
-    ZKB_TRY(ntt_fr_device(ctx, h_ext, h_ext, pk->ext_k, pk->ext_omega_inv, &pk->N_inv, 2, nullptr, st));
-    {
-        std::vector<Fr *> pcs;
-        for (uint32_t i = 0; i < pk->qdeg; ++i) pcs.push_back(h_ext + (size_t)i * n);
-        std::vector<G1Affine> cms;
-        ZKB_TRY(commit_many(pk, pcs, pk->g, n, cms, st));
-        for (auto &cm : cms) ZKB_TRY(tr_write_point(s, cm));
-    }
-    const Fr x = tr_squeeze(s);
-    const Fr xn = fp_pow_u64(x, n);
+    return ZKB_OK;
+}
 
-    trace.mark("extended iNTT + h commits");
-    // ---------------------------------------------------------------- evaluations (prover.rs order)
+// vanishing/prover.rs construct: extended_to_coeff (inverse NTT over the extended domain with 1/N and the zeta coset undone), the
+// qdeg pieces of n coefficients committed against g, then x
+static int32_t vanishing_construct(zkb_session *s, ProofState &ps) {
+    zkb_pk *pk = s->pk;
+    cudaStream_t st = pk->ctx->stream;
+    ZKB_TRY(ntt_fr_device(pk->ctx, ps.h_ext, ps.h_ext, pk->ext_k, pk->ext_omega_inv, &pk->N_inv, 2, nullptr, st));
+    for (uint32_t i = 0; i < pk->qdeg; ++i) ps.h_pieces.push_back(ps.h_ext + (size_t)i * pk->n);
+    ZKB_TRY(commit_write(s, ps.h_pieces, BASIS_G, st));
+    ps.x = tr_squeeze(s);
+    return ZKB_OK;
+}
+
+// prover.rs evaluations (with permutation / mv_lookup / vanishing evaluate), batched per rotation and written in upstream's order;
+// then the multiopen query list in prover.rs order
+static int32_t evaluate_at_x(zkb_session *s, ProofState &ps) {
+    zkb_pk *pk = s->pk;
+    zkb_ctx *ctx = pk->ctx;
+    const Csf &cs = pk->cs;
+    const uint64_t n = pk->n;
+    const size_t nl = cs.lookups.size();
+    cudaStream_t st = ctx->stream;
+    DevPool &pool = s->pool;
     // h(X) = sum_i x^(n i) piece_i
     Fr *h_poly;
     ZKB_TRY(pool.fr(n, &h_poly));
     {
-        std::vector<Fr *> pcs;
+        const Fr xn = fp_pow_u64(ps.x, n);
         std::vector<Fr> cf;
-        Fr cur = one;
-        for (uint32_t i = 0; i < pk->qdeg; ++i) { pcs.push_back(h_ext + (size_t)i * n); cf.push_back(cur); cur = fp_mul(cur, xn); }
-        Fr **d_p = nullptr;
-        Fr *d_c = nullptr;
-        ZKB_TRY(upload_table(pool, pcs, &d_p, st));
-        ZKB_TRY(pool.fr(cf.size(), &d_c));
-        ZKB_CUDA(cudaMemcpyAsync(d_c, cf.data(), cf.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
-        ZKB_TRY(lincomb_device(ctx, d_p, d_c, (uint32_t)pcs.size(), n, h_poly, false, st));
+        Fr cur = Fr::one();
+        for (uint32_t i = 0; i < pk->qdeg; ++i) { cf.push_back(cur); cur = fp_mul(cur, xn); }
+        ZKB_TRY(lincomb(pk, pool, ps.h_pieces, cf, h_poly, false, st));
         ZKB_CUDA(cudaStreamSynchronize(st));
     }
-    std::vector<OpenQuery> queries;
     int next_id = 0;
     std::vector<int> adv_id(cs.na), fix_id(cs.nf), sig_id(cs.perm.size()), z_id(pk->nsets), phi_id(nl), m_id(nl);
     for (auto &v : adv_id) v = next_id++;
@@ -1556,23 +1548,23 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
     for (auto &v : phi_id) v = next_id++;
     for (auto &v : m_id) v = next_id++;
     const int h_id = next_id++, rand_id = next_id++;
-    const int64_t rot_last = -(int64_t)(bf + 1);
+    const int64_t rot_last = -(int64_t)(cs.bf + 1);
     // (1) the evaluations written to the transcript, in order; `queries` is built afterwards in the multiopen order
     struct EvalReq { int poly_id; const Fr *poly; int64_t rot; };
     std::vector<EvalReq> reqs;
-    for (auto &q : cs.advq) reqs.push_back({adv_id[q[0]], adv_polys[q[0]], q[1]});
+    for (auto &q : cs.advq) reqs.push_back({adv_id[q[0]], ps.adv_polys[q[0]], q[1]});
     for (auto &q : cs.fixq) reqs.push_back({fix_id[q[0]], pk->fixed_polys[q[0]], q[1]});
-    reqs.push_back({rand_id, random_poly, 0});
+    reqs.push_back({rand_id, ps.random_poly, 0});
     for (size_t i = 0; i < cs.perm.size(); ++i) reqs.push_back({sig_id[i], pk->sigma_polys[i], 0});
     for (uint32_t i = 0; i < pk->nsets; ++i) {
-        reqs.push_back({z_id[i], z_polys[i], 0});
-        reqs.push_back({z_id[i], z_polys[i], 1});
-        if (i + 1 != pk->nsets) reqs.push_back({z_id[i], z_polys[i], rot_last});
+        reqs.push_back({z_id[i], ps.z_polys[i], 0});
+        reqs.push_back({z_id[i], ps.z_polys[i], 1});
+        if (i + 1 != pk->nsets) reqs.push_back({z_id[i], ps.z_polys[i], rot_last});
     }
     for (size_t l = 0; l < nl; ++l) {
-        reqs.push_back({phi_id[l], phi_polys[l], 0});
-        reqs.push_back({phi_id[l], phi_polys[l], 1});
-        reqs.push_back({m_id[l], m_polys[l], 0});
+        reqs.push_back({phi_id[l], ps.phi_polys[l], 0});
+        reqs.push_back({phi_id[l], ps.phi_polys[l], 1});
+        reqs.push_back({m_id[l], ps.m_polys[l], 0});
     }
     const size_t n_written = reqs.size();
     reqs.push_back({h_id, h_poly, 0});  // needed by SHPLONK, not written
@@ -1580,10 +1572,9 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
     std::map<int64_t, std::vector<size_t>> by_rot;
     for (size_t i = 0; i < reqs.size(); ++i) by_rot[reqs[i].rot].push_back(i);
     std::vector<Fr> evals(reqs.size());
-    std::map<int64_t, Fr> point_of;
     for (auto &kv : by_rot) {
-        const Fr pt = fp_mul(x, fr_pow_i64(pk->omega, pk->omega_inv, kv.first));
-        point_of[kv.first] = pt;
+        const Fr pt = fp_mul(ps.x, fr_pow_i64(pk->omega, pk->omega_inv, kv.first));
+        ps.point_of[kv.first] = pt;
         std::vector<Fr *> ptrs;
         for (size_t i : kv.second) ptrs.push_back(const_cast<Fr *>(reqs[i].poly));
         Fr **d_p = nullptr;
@@ -1606,34 +1597,70 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
         for (size_t t = 0; t < kv.second.size(); ++t) evals[kv.second[t]] = res[t];
     }
     for (size_t i = 0; i < n_written; ++i) tr_write_scalar(s, evals[i]);
-    std::map<std::pair<int, int64_t>, Fr> eval_of;
-    for (size_t i = 0; i < reqs.size(); ++i) eval_of[{reqs[i].poly_id, reqs[i].rot}] = evals[i];
+    for (size_t i = 0; i < reqs.size(); ++i) ps.eval_of[{reqs[i].poly_id, reqs[i].rot}] = evals[i];
 
     // (2) multiopen queries in prover.rs order
-    auto push_q = [&](int id, const Fr *poly, int64_t rot) { queries.push_back({id, poly, rot, point_of[rot], eval_of[{id, rot}]}); };
-    for (auto &q : cs.advq) push_q(adv_id[q[0]], adv_polys[q[0]], q[1]);
-    for (uint32_t i = 0; i < pk->nsets; ++i) { push_q(z_id[i], z_polys[i], 0); push_q(z_id[i], z_polys[i], 1); }
-    for (int i = (int)pk->nsets - 2; i >= 0; --i) push_q(z_id[i], z_polys[i], rot_last);
-    for (size_t l = 0; l < nl; ++l) { push_q(phi_id[l], phi_polys[l], 0); push_q(phi_id[l], phi_polys[l], 1); push_q(m_id[l], m_polys[l], 0); }
+    auto push_q = [&](int id, const Fr *poly, int64_t rot) { ps.queries.push_back({id, poly, rot}); };
+    for (auto &q : cs.advq) push_q(adv_id[q[0]], ps.adv_polys[q[0]], q[1]);
+    for (uint32_t i = 0; i < pk->nsets; ++i) { push_q(z_id[i], ps.z_polys[i], 0); push_q(z_id[i], ps.z_polys[i], 1); }
+    for (int i = (int)pk->nsets - 2; i >= 0; --i) push_q(z_id[i], ps.z_polys[i], rot_last);
+    for (size_t l = 0; l < nl; ++l) { push_q(phi_id[l], ps.phi_polys[l], 0); push_q(phi_id[l], ps.phi_polys[l], 1); push_q(m_id[l], ps.m_polys[l], 0); }
     for (auto &q : cs.fixq) push_q(fix_id[q[0]], pk->fixed_polys[q[0]], q[1]);
     for (size_t i = 0; i < cs.perm.size(); ++i) push_q(sig_id[i], pk->sigma_polys[i], 0);
     push_q(h_id, h_poly, 0);
-    push_q(rand_id, random_poly, 0);
+    push_q(rand_id, ps.random_poly, 0);
+    return ZKB_OK;
+}
 
-    trace.mark("evaluations");
-    // ---------------------------------------------------------------- SHPLONK (multiopen/shplonk/prover.rs)
+// low-degree interpolant through (points, evals): coefficients, low to high
+static std::vector<Fr> interpolate(const std::vector<Fr> &pts, const std::vector<Fr> &evs) {
+    const size_t m = pts.size();
+    std::vector<Fr> coeffs(m, Fr::zero());
+    for (size_t j = 0; j < m; ++j) {
+        std::vector<Fr> num{Fr::one()};
+        Fr den = Fr::one();
+        for (size_t t = 0; t < m; ++t) {
+            if (t == j) continue;
+            std::vector<Fr> nx(num.size() + 1, Fr::zero());
+            for (size_t i = 0; i < num.size(); ++i) {
+                nx[i + 1] = fp_add(nx[i + 1], num[i]);
+                nx[i] = fp_sub(nx[i], fp_mul(pts[t], num[i]));
+            }
+            num.swap(nx);
+            den = fp_mul(den, fp_sub(pts[j], pts[t]));
+        }
+        const Fr sc = fp_mul(evs[j], fp_inv(den));
+        for (size_t i = 0; i < m; ++i) coeffs[i] = fp_add(coeffs[i], fp_mul(num[i], sc));
+    }
+    return coeffs;
+}
+static Fr horner_host(const std::vector<Fr> &c, const Fr &at) {
+    Fr acc = Fr::zero();
+    for (size_t i = c.size(); i-- > 0;) acc = fp_add(fp_mul(acc, at), c[i]);
+    return acc;
+}
+
+// multiopen/shplonk/prover.rs: rotation sets (construct_intermediate_sets), numerators sum_j y^j (P_ij - R_ij) divided by each
+// set's vanishing polynomial into h_x, its commitment, then the linearisation at u divided by (X - u) and the final commitment
+static int32_t shplonk(zkb_session *s, ProofState &ps) {
+    zkb_pk *pk = s->pk;
+    zkb_ctx *ctx = pk->ctx;
+    const uint64_t n = pk->n;
+    const Fr one = Fr::one();
+    cudaStream_t st = ctx->stream;
+    DevPool &pool = s->pool;
     const Fr sy = tr_squeeze(s);
     // construct_intermediate_sets
     struct Commit { int id; const Fr *poly; std::vector<int64_t> rots; };
     std::vector<Commit> cmap;
     std::vector<int64_t> super_rots;
-    for (auto &q : queries) {
+    for (auto &q : ps.queries) {
         if (std::find(super_rots.begin(), super_rots.end(), q.rot) == super_rots.end()) super_rots.push_back(q.rot);
         auto it = std::find_if(cmap.begin(), cmap.end(), [&](const Commit &c) { return c.id == q.poly_id; });
         if (it == cmap.end()) cmap.push_back({q.poly_id, q.poly, {q.rot}});
         else if (std::find(it->rots.begin(), it->rots.end(), q.rot) == it->rots.end()) it->rots.push_back(q.rot);
     }
-    auto sort_rots = [&](std::vector<int64_t> &r) { std::sort(r.begin(), r.end(), [&](int64_t a, int64_t b) { return fr_less(point_of[a], point_of[b]); }); };
+    auto sort_rots = [&](std::vector<int64_t> &r) { std::sort(r.begin(), r.end(), [&](int64_t a, int64_t b) { return fr_less(ps.point_of[a], ps.point_of[b]); }); };
     sort_rots(super_rots);
     for (auto &c : cmap) sort_rots(c.rots);
     struct RSet { std::vector<int64_t> rots; std::vector<Commit *> comms; };
@@ -1644,145 +1671,115 @@ static int32_t prove_finish_impl(zkb_session *s, const uint64_t *z_blinds, const
         else it->comms.push_back(&c);
     }
     const Fr sv = tr_squeeze(s);
-    // low-degree interpolant through (points, evals): coefficients, low to high
-    auto interpolate = [&](const std::vector<Fr> &pts, const std::vector<Fr> &evs) {
-        const size_t m = pts.size();
-        std::vector<Fr> coeffs(m, Fr::zero());
-        for (size_t j = 0; j < m; ++j) {
-            std::vector<Fr> num{one};
-            Fr den = one;
-            for (size_t t = 0; t < m; ++t) {
-                if (t == j) continue;
-                std::vector<Fr> nx(num.size() + 1, Fr::zero());
-                for (size_t i = 0; i < num.size(); ++i) {
-                    nx[i + 1] = fp_add(nx[i + 1], num[i]);
-                    nx[i] = fp_sub(nx[i], fp_mul(pts[t], num[i]));
-                }
-                num.swap(nx);
-                den = fp_mul(den, fp_sub(pts[j], pts[t]));
-            }
-            const Fr sc = fp_mul(evs[j], fp_inv(den));
-            for (size_t i = 0; i < m; ++i) coeffs[i] = fp_add(coeffs[i], fp_mul(num[i], sc));
-        }
-        return coeffs;
-    };
-    auto horner_host = [&](const std::vector<Fr> &c, const Fr &at) {
-        Fr acc = Fr::zero();
-        for (size_t i = c.size(); i-- > 0;) acc = fp_add(fp_mul(acc, at), c[i]);
-        return acc;
-    };
     Fr *hx, *work, *work2, *d_small;
     ZKB_TRY(pool.fr(n, &hx));
     ZKB_TRY(pool.fr(n, &work));
     ZKB_TRY(pool.fr(n, &work2));
     ZKB_TRY(pool.fr(256, &d_small));
     ZKB_CUDA(cudaMemsetAsync(hx, 0, n * sizeof(Fr), st));
-    struct SetData { std::vector<Fr> pts; std::vector<std::vector<Fr>> r_coeffs; };
-    std::vector<SetData> sdata(rsets.size());
-    {
-        Fr vpow = one;
-        for (size_t si = 0; si < rsets.size(); ++si) {
-            RSet &rs = rsets[si];
-            SetData &sd = sdata[si];
-            for (int64_t r : rs.rots) sd.pts.push_back(point_of[r]);
-            ZKB_ARG(sd.pts.size() <= 256);   // Keccak's hot cell column is opened at 56 rotations (keccak_packed_multi.rs:59-68)
-            // N_i(X) = sum_j y^j (P_ij(X) - R_ij(X))
-            std::vector<Fr *> ptrs;
-            std::vector<Fr> cf;
-            std::vector<Fr> rsum(sd.pts.size(), Fr::zero());
-            Fr ypow = one;
-            for (Commit *c : rs.comms) {
-                std::vector<Fr> evs;
-                for (int64_t r : rs.rots) evs.push_back(eval_of[{c->id, r}]);
-                sd.r_coeffs.push_back(interpolate(sd.pts, evs));
-                for (size_t i = 0; i < sd.pts.size(); ++i) rsum[i] = fp_add(rsum[i], fp_mul(sd.r_coeffs.back()[i], ypow));
-                ptrs.push_back(const_cast<Fr *>(c->poly));
-                cf.push_back(ypow);
-                ypow = fp_mul(ypow, sy);
-            }
-            Fr **d_p = nullptr;
-            Fr *d_c = nullptr;
-            ZKB_TRY(upload_table(pool, ptrs, &d_p, st));
-            ZKB_TRY(pool.fr(cf.size(), &d_c));
-            ZKB_CUDA(cudaMemcpyAsync(d_c, cf.data(), cf.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
-            ZKB_TRY(lincomb_device(ctx, d_p, d_c, (uint32_t)ptrs.size(), n, work, false, st));
-            ZKB_CUDA(cudaMemcpyAsync(d_small, rsum.data(), rsum.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
-            sub_low_kernel<<<1, 256, 0, st>>>(work, d_small, (uint32_t)rsum.size());
-            ctx->launches++;
-            ZKB_CUDA(cudaStreamSynchronize(st));
-            // divide by the vanishing polynomial of the set, one root at a time
-            Fr *src = work, *dst = work2;
-            for (const Fr &p : sd.pts) {
-                ZKB_TRY(kate_division_device(ctx, src, n, p, dst, st));
-                std::swap(src, dst);
-            }
-            // h_x += v^i * Q_i
-            std::vector<Fr *> one_ptr{src};
-            Fr **d_q = nullptr;
-            Fr *d_v = nullptr;
-            ZKB_TRY(upload_table(pool, one_ptr, &d_q, st));
-            ZKB_TRY(pool.fr(1, &d_v));
-            ZKB_CUDA(cudaMemcpyAsync(d_v, &vpow, sizeof(Fr), cudaMemcpyHostToDevice, st));
-            ZKB_TRY(lincomb_device(ctx, d_q, d_v, 1, n, hx, true, st));
-            ZKB_CUDA(cudaStreamSynchronize(st));
-            vpow = fp_mul(vpow, sv);
-        }
-    }
-    {
-        G1Affine cm;
-        { std::vector<Fr *> one_col{hx}; std::vector<G1Affine> r1; ZKB_TRY(commit_many(pk, one_col, pk->g, n, r1, st)); cm = r1[0]; }
-        ZKB_TRY(tr_write_point(s, cm));
-    }
-    const Fr su = tr_squeeze(s);
-    {
-        // L(X) = sum_i v^i z_i sum_j y^j (P_ij(X) - r_ij) - zt * h_x(X), scaled by 1/z_0, divided by (X - u)
-        std::vector<Fr> super_pts;
-        for (int64_t r : super_rots) super_pts.push_back(point_of[r]);
-        std::vector<Fr> zdiff(rsets.size());
-        for (size_t si = 0; si < rsets.size(); ++si) {
-            Fr z = one;
-            for (size_t t = 0; t < super_rots.size(); ++t) {
-                if (std::find(rsets[si].rots.begin(), rsets[si].rots.end(), super_rots[t]) == rsets[si].rots.end()) z = fp_mul(z, fp_sub(su, super_pts[t]));
-            }
-            zdiff[si] = z;
-        }
-        Fr zt = one;
-        for (auto &p : super_pts) zt = fp_mul(zt, fp_sub(su, p));
-        const Fr z0inv = fp_inv(zdiff[0]);
+    std::vector<std::vector<std::vector<Fr>>> r_coeffs(rsets.size());   // [set][commitment] -> interpolant R_ij
+    Fr vpow = one;
+    for (size_t si = 0; si < rsets.size(); ++si) {
+        const RSet &rs = rsets[si];
+        std::vector<Fr> pts;
+        for (int64_t r : rs.rots) pts.push_back(ps.point_of[r]);
+        ZKB_ARG(pts.size() <= 256);   // Keccak's hot cell column is opened at 56 rotations (keccak_packed_multi.rs:59-68)
+        // N_i(X) = sum_j y^j (P_ij(X) - R_ij(X))
         std::vector<Fr *> ptrs;
         std::vector<Fr> cf;
-        Fr const_term = Fr::zero();
-        Fr vpow = one;
-        for (size_t si = 0; si < rsets.size(); ++si) {
-            Fr ypow = one;
-            for (size_t ci = 0; ci < rsets[si].comms.size(); ++ci) {
-                const Fr w = fp_mul(fp_mul(fp_mul(vpow, zdiff[si]), ypow), z0inv);
-                ptrs.push_back(const_cast<Fr *>(rsets[si].comms[ci]->poly));
-                cf.push_back(w);
-                const_term = fp_add(const_term, fp_mul(w, horner_host(sdata[si].r_coeffs[ci], su)));
-                ypow = fp_mul(ypow, sy);
-            }
-            vpow = fp_mul(vpow, sv);
+        std::vector<Fr> rsum(pts.size(), Fr::zero());
+        Fr ypow = one;
+        for (Commit *c : rs.comms) {
+            std::vector<Fr> evs;
+            for (int64_t r : rs.rots) evs.push_back(ps.eval_of[{c->id, r}]);
+            r_coeffs[si].push_back(interpolate(pts, evs));
+            for (size_t i = 0; i < pts.size(); ++i) rsum[i] = fp_add(rsum[i], fp_mul(r_coeffs[si].back()[i], ypow));
+            ptrs.push_back(const_cast<Fr *>(c->poly));
+            cf.push_back(ypow);
+            ypow = fp_mul(ypow, sy);
         }
-        ptrs.push_back(hx);
-        cf.push_back(fp_neg(fp_mul(zt, z0inv)));
-        Fr **d_p = nullptr;
-        Fr *d_c = nullptr;
-        ZKB_TRY(upload_table(pool, ptrs, &d_p, st));
-        ZKB_TRY(pool.fr(cf.size(), &d_c));
-        ZKB_CUDA(cudaMemcpyAsync(d_c, cf.data(), cf.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
-        ZKB_TRY(lincomb_device(ctx, d_p, d_c, (uint32_t)ptrs.size(), n, work, false, st));
-        ZKB_CUDA(cudaMemcpyAsync(d_small, &const_term, sizeof(Fr), cudaMemcpyHostToDevice, st));
-        sub_low_kernel<<<1, 256, 0, st>>>(work, d_small, 1);
+        ZKB_TRY(lincomb(pk, pool, ptrs, cf, work, false, st));
+        ZKB_CUDA(cudaMemcpyAsync(d_small, rsum.data(), rsum.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
+        sub_low_kernel<<<1, 256, 0, st>>>(work, d_small, (uint32_t)rsum.size());
         ctx->launches++;
         ZKB_CUDA(cudaStreamSynchronize(st));
-        ZKB_TRY(kate_division_device(ctx, work, n, su, work2, st));
-        G1Affine cm;
-        { std::vector<Fr *> one_col{work2}; std::vector<G1Affine> r1; ZKB_TRY(commit_many(pk, one_col, pk->g, n, r1, st)); cm = r1[0]; }
-        ZKB_TRY(tr_write_point(s, cm));
+        // divide by the vanishing polynomial of the set, one root at a time
+        Fr *src = work, *dst = work2;
+        for (const Fr &p : pts) {
+            ZKB_TRY(kate_division_device(ctx, src, n, p, dst, st));
+            std::swap(src, dst);
+        }
+        // h_x += v^i * Q_i
+        const std::vector<Fr> vcoef{vpow};
+        ZKB_TRY(lincomb(pk, pool, {src}, vcoef, hx, true, st));
+        ZKB_CUDA(cudaStreamSynchronize(st));
+        vpow = fp_mul(vpow, sv);
     }
+    ZKB_TRY(commit_write(s, {hx}, BASIS_G, st));
+    const Fr su = tr_squeeze(s);
+    // L(X) = sum_i v^i z_i sum_j y^j (P_ij(X) - r_ij) - zt * h_x(X), scaled by 1/z_0, divided by (X - u)
+    std::vector<Fr> super_pts;
+    for (int64_t r : super_rots) super_pts.push_back(ps.point_of[r]);
+    std::vector<Fr> zdiff(rsets.size());
+    for (size_t si = 0; si < rsets.size(); ++si) {
+        Fr z = one;
+        for (size_t t = 0; t < super_rots.size(); ++t) {
+            if (std::find(rsets[si].rots.begin(), rsets[si].rots.end(), super_rots[t]) == rsets[si].rots.end()) z = fp_mul(z, fp_sub(su, super_pts[t]));
+        }
+        zdiff[si] = z;
+    }
+    Fr zt = one;
+    for (auto &p : super_pts) zt = fp_mul(zt, fp_sub(su, p));
+    const Fr z0inv = fp_inv(zdiff[0]);
+    std::vector<Fr *> ptrs;
+    std::vector<Fr> cf;
+    Fr const_term = Fr::zero();
+    vpow = one;
+    for (size_t si = 0; si < rsets.size(); ++si) {
+        Fr ypow = one;
+        for (size_t ci = 0; ci < rsets[si].comms.size(); ++ci) {
+            const Fr w = fp_mul(fp_mul(fp_mul(vpow, zdiff[si]), ypow), z0inv);
+            ptrs.push_back(const_cast<Fr *>(rsets[si].comms[ci]->poly));
+            cf.push_back(w);
+            const_term = fp_add(const_term, fp_mul(w, horner_host(r_coeffs[si][ci], su)));
+            ypow = fp_mul(ypow, sy);
+        }
+        vpow = fp_mul(vpow, sv);
+    }
+    ptrs.push_back(hx);
+    cf.push_back(fp_neg(fp_mul(zt, z0inv)));
+    ZKB_TRY(lincomb(pk, pool, ptrs, cf, work, false, st));
+    ZKB_CUDA(cudaMemcpyAsync(d_small, &const_term, sizeof(Fr), cudaMemcpyHostToDevice, st));
+    sub_low_kernel<<<1, 256, 0, st>>>(work, d_small, 1);
+    ctx->launches++;
+    ZKB_CUDA(cudaStreamSynchronize(st));
+    ZKB_TRY(kate_division_device(ctx, work, n, su, work2, st));
+    return commit_write(s, {work2}, BASIS_G, st);
+}
+
+// create_proof after the advice phases (plonk/prover.rs), one function per upstream stage, in transcript order
+static int32_t prove_finish_stages(zkb_session *s, const uint64_t *z_blinds, const uint64_t *phi_blinds, const uint64_t *random_poly_host) {
+    ProofState ps;
+    StageTrace trace(s->pk->ctx->stream);
+    ZKB_TRY(lookup_prepare(s, ps));
+    trace.mark("lookups: compress + m + commit");
+    ZKB_TRY(permutation_commit(s, ps, z_blinds));
+    trace.mark("permutation z + commit");
+    ZKB_TRY(lookup_commit_grand_sum(s, ps, phi_blinds));
+    trace.mark("lookup phi + commit");
+    ZKB_TRY(vanishing_commit(s, ps, random_poly_host));
+    trace.mark("random poly commit");
+    ZKB_TRY(coefficient_forms(s, ps));
+    trace.mark("lagrange_to_coeff (all columns)");
+    ZKB_TRY(evaluate_h(s, ps, trace));   // marks "quotient program build+upload" between the program and the coset parts
+    trace.mark("quotient: coset NTTs + fused eval");
+    ZKB_TRY(vanishing_construct(s, ps));
+    trace.mark("extended iNTT + h commits");
+    ZKB_TRY(evaluate_at_x(s, ps));
+    trace.mark("evaluations");
+    ZKB_TRY(shplonk(s, ps));
     trace.mark("shplonk");
-    if (s->cb_error) { set_error("the caller's transcript callback failed (%d)", s->cb_error); return ZKB_ERR_STATE; }
+    ZKB_TRY(callback_status(s));
     s->finished = true;
     return ZKB_OK;
 }
@@ -1800,7 +1797,7 @@ extern "C" int32_t zkb_prove_finish(zkb_session *s, const uint64_t *z_blinds, co
         if (s->next_phase != pk->cs.nphases) { set_error("zkb_prove_finish: advice phases incomplete"); return ZKB_ERR_STATE; }
         ZKB_ARG((pk->nsets == 0 || z_blinds) && (pk->cs.lookups.empty() || phi_blinds));
         ZKB_CUDA(cudaSetDevice(pk->ctx->device));
-        ZKB_TRY(prove_finish_impl(s, z_blinds, phi_blinds, random_poly));
+        ZKB_TRY(prove_finish_stages(s, z_blinds, phi_blinds, random_poly));
     }
     *proof_len = s->proof.size();
     if (proof_out) {
