@@ -238,6 +238,19 @@ ZKB_API int32_t zkb_pk_destroy(zkb_pk *pk);
 ZKB_API int32_t zkb_pk_vk_bytes(zkb_pk *pk, uint8_t *out, uint64_t cap, uint64_t *len);
 /* Host-only structural validation of a CSF blob (no CUDA device needed); zkb_pk_create runs it first.                       */
 ZKB_API int32_t zkb_csf_validate(const uint32_t *csf, uint64_t csf_words);
+/* The gates of a CSF evaluated over caller columns by the prover's own expression compiler and interpreter (the quotient's hot
+ * kernel, exposed for row-by-row tests).  columns_dev: HOST array of device pointers in slot order fixed | advice | instance,
+ * 2^k elements each; challenges: num_challenges x 4 limbs (Montgomery), may be NULL without challenges.
+ *   mode 0: gate i -> outs_dev[i][row], all gates in ONE common-subexpression scope (like the lookup compression programs);
+ *           out_stride must be 1 and out_offset 0.
+ *   mode 1: the gates folded in y exactly as the quotient program of zkb_prove_finish (selector runs folded), times `scale`,
+ *           -> outs_dev[0][row * out_stride + out_offset]; other entries are not written.
+ * *nregs_out (may be NULL) receives the register count that chose the kernel build (<= 8, <= 16: shared memory; <= 64: local
+ * memory).  A program needing more than 64 live registers fails with ZKB_ERR_ARG before anything is launched.  Synchronises
+ * `stream`.                                                                                                                  */
+ZKB_API int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, int32_t mode, const uint64_t *challenges,
+                                  const uint64_t y[4], const uint64_t scale[4], const uint64_t *const *columns_dev,
+                                  uint64_t *const *outs_dev, uint32_t out_stride, uint32_t out_offset, uint32_t *nregs_out, void *stream);
 ZKB_API int32_t zkb_prove_begin(zkb_pk *pk, const uint64_t transcript_repr[4], const uint64_t *const *instance_values,
                                 const uint32_t *instance_lens, zkb_session **out);
 /* Same with a choice of transcript: 0 = Blake2bWrite/Challenge255 (the reference's benches, circuit-benchmarks/src/super_circuit.rs:112),

@@ -237,3 +237,47 @@ class GatesOnlyCircuit:
         for c in range(2):
             v = list(self.cols[c]); v[self.usable:] = self.blind_rows[c]; out[c] = v
         return out
+
+
+class DeepGateCircuit:
+    """One deep gate whose quotient program needs more than 16 live registers, so the proof runs the interpreter's local-memory
+    build: q * (a_0 * a_0(1) * a_1 * a_1(1) * ... * a_{m-1}(1) - a_m), the product nested to the right (2m queries live at
+    once next to q), plus a permutation over a_0 and a_1 with copies that hold.  fixed: 0 q;  advice: 0 .. m."""
+
+    def __init__(self, k, seed=0, m=8):
+        rnd = random.Random(seed)
+        self.k, self.n = k, 1 << k
+        n = self.n
+        cs = H.ConstraintSystem(k, 1, m + 1, 0)
+        queries = [H.advice(c, r) for c in range(m) for r in (0, 1)]
+        prod = queries[-1]
+        for e in reversed(queries[:-1]):
+            prod = e * prod
+        cs.gates.append(H.fixed(0) * (prod - H.advice(m)))
+        cs.perm_columns = [(ADVICE, 0), (ADVICE, 1)]
+        cs.finalize()
+        self.cs = cs
+        bf = cs.blinding_factors()
+        usable = n - (bf + 1)
+        self.usable = usable
+        cols = [[rnd.randrange(R) for _ in range(n)] for _ in range(m + 1)]   # rows >= usable are the blinding rows
+        copies = []
+        for i in rnd.sample(range(usable), max(1, usable // 8)):             # a_1[i] = a_0[j]: decided before the product
+            j = rnd.randrange(usable)
+            cols[1][i] = cols[0][j]; copies.append(((ADVICE, 1, i), (ADVICE, 0, j)))
+        q = [1 if i < usable - 1 and rnd.random() < 0.8 else 0 for i in range(n)]
+        for i in range(n):
+            if q[i]:
+                v = 1
+                for c in range(m):
+                    v = v * cols[c][i] % R * cols[c][i + 1] % R
+                cols[m][i] = v
+        self.fixed_ints, self.copies, self.instances = [q], copies, []
+        self.cols = cols
+        nsets = (len(cs.perm_columns) + (cs.degree() - 2) - 1) // (cs.degree() - 2)
+        self.blinds_ints = {"z": [[rnd.randrange(R) for _ in range(bf)] for _ in range(nsets)], "phi": [],
+                            "random_poly": [rnd.randrange(R) for _ in range(n)]}
+        self.transcript_repr = rnd.randrange(R)
+
+    def advice_ints(self, phase, challenges):
+        return {c: list(v) for c, v in enumerate(self.cols)}

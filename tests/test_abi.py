@@ -27,6 +27,27 @@ def test_version():
     assert zkb200.load_library().zkb_version() >> 16 == 1
 
 
+def test_handles_outliving_their_context_are_not_destroyed():
+    """Finalisers of garbage run in no fixed order: at interpreter exit the traceback of a failed proof test can keep a proving key
+    alive past its context.  A key or SRS whose context is already destroyed must not reach zkb_pk_destroy / zkb_srs_destroy,
+    which would read the freed context (a crash at exit)."""
+    from zkb200 import lib as zl, plonk as Z, params
+    calls = []
+
+    class Lib:
+        def __getattr__(self, name): return lambda *a: calls.append(name)
+    ctx = zl.Context.__new__(zl.Context)
+    ctx.lib, ctx.handle = Lib(), 1
+    objs = [Z.ProvingKey.__new__(Z.ProvingKey), params.Srs.__new__(params.Srs), Z.ProvingKey.__new__(Z.ProvingKey)]
+    for o in objs:
+        o.ctx, o.handle = ctx, 2
+    objs[0].close()
+    ctx.close()
+    objs[1].close(); objs[2].close()
+    assert calls == ["zkb_pk_destroy", "zkb_destroy"]
+    assert all(o.handle is None for o in objs)
+
+
 def test_root_of_unity_matches_fixture(golden):
     import numpy as np
     from zkb200 import arithmetic
@@ -73,6 +94,23 @@ def test_csf_roundtrip_and_validation():
             Z.validate_csf(bad)
     with pytest.raises(zkb200.ZkbError):
         Z.validate_csf(blob[:20])
+
+
+def test_csf_rotation_limit():
+    """The interpreter keeps a rotation in 16 bits: +-32767 is accepted, +-32768 is rejected, in a gate and in the query list."""
+    import zkb200
+    from zkb200 import plonk as Z
+    E = Z.Expression
+    for rot in (32767, -32767, 32768, -32768):
+        for in_gate in (True, False):
+            cs = Z.ConstraintSystem(3, 1, 1, 0, [0], [], 5, 3)
+            cs.gates = [E.Fixed(0) * E.Advice(0, rot if in_gate else 0)]
+            cs.advice_queries = [(0, 0 if in_gate else rot)]
+            if abs(rot) <= 32767:
+                Z.validate_csf(cs.to_csf())
+            else:
+                with pytest.raises(zkb200.ZkbError, match="16 bits"):
+                    Z.validate_csf(cs.to_csf())
 
 
 def test_params_file_roundtrip(tmp_path, oracle):

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 import halo2_ref as H
-from circuits import ToyCircuit, ThinCompressionShape, GatesOnlyCircuit
+from circuits import ToyCircuit, ThinCompressionShape, GatesOnlyCircuit, DeepGateCircuit
 
 pytestmark = pytest.mark.gpu
 
@@ -40,13 +40,13 @@ def first_diff(a, b):
 
 
 CASES = [("toy", 5, {}), ("toy", 6, dict(two_phase=False)), ("toy", 6, dict(lookups=False, extra_perm=False)), ("toy", 8, {}), ("toy", 11, {}),
-         ("thin", 7, {}), ("thin", 10, {}), ("gates", 5, {}), ("gates", 9, {})]
+         ("thin", 7, {}), ("thin", 10, {}), ("gates", 5, {}), ("gates", 9, {}), ("deep", 6, {}), ("deep", 9, {})]
 
 
 @pytest.mark.parametrize("kind,k,kw", CASES)
 def test_create_proof_matches_oracle(kind, k, kw):
     from zkb200 import plonk as Z
-    tc = {"toy": ToyCircuit, "thin": ThinCompressionShape, "gates": GatesOnlyCircuit}[kind](k, seed=100 + k, **kw)
+    tc = {"toy": ToyCircuit, "thin": ThinCompressionShape, "gates": GatesOnlyCircuit, "deep": DeepGateCircuit}[kind](k, seed=100 + k, **kw)
     ref = H.Ref(tc.cs, 1234)
     F = ref.F
     fixed = [F.arr(c) for c in tc.fixed_ints]
@@ -69,6 +69,14 @@ def test_create_proof_matches_oracle(kind, k, kw):
     assert len(proof) == len(proof_ref)
     assert first_diff(proof, proof_ref) is None, f"first differing 32-byte proof item: {first_diff(proof, proof_ref)}"
     assert ref.verify_proof(pkr, tc.transcript_repr, tc.instances, proof)
+    if kind == "deep":
+        # the quotient program's register count is the maximum over its scopes: its gate part alone needs the local-memory build
+        # (> 16 registers), so the proof above ran expr_kernel<64, 128, false>.  On the satisfied witness the folded gate is zero.
+        import torch
+        cols = [torch.from_numpy(np.ascontiguousarray(c).view(np.int64)).cuda() for c in fixed + [F.arr(v) for v in tc.advice_ints(0, {}).values()]]
+        (h,), nregs = Z.expr_eval(zcs, cols, mode=1, y=F.arr([5])[0], scale=F.arr([1])[0])
+        assert nregs >= 17
+        assert not h.cpu().numpy().any()
 
 
 def test_unsatisfied_lookup_is_reported():

@@ -465,18 +465,21 @@ static int32_t upload_table(DevPool &pool, const std::vector<T *> &host, T ***de
     ZKB_CUDA(cudaStreamSynchronize(st));
     return ZKB_OK;
 }
-// one program whose root i is STOREd to outs[i], uploaded with its output table and run over the n rows of the d_cols table
-static int32_t run_store_program(zkb_pk *pk, DevPool &pool, ExprBuilder &eb, const std::vector<uint32_t> &roots, const std::vector<Fr *> &outs,
-                                 const Fr *const *d_cols, const std::string &what, cudaStream_t st) {
+// one program whose root i is STOREd to outs[i], uploaded with its output table and run over the 2^log_n rows of the d_cols table;
+// *nregs (if given) receives the program's register count
+static int32_t run_store_program(zkb_ctx *ctx, uint32_t log_n, DevPool &pool, ExprBuilder &eb, const std::vector<uint32_t> &roots,
+                                 const std::vector<Fr *> &outs, const Fr *const *d_cols, const std::string &what, cudaStream_t st,
+                                 int *nregs = nullptr) {
     ProgramBuilder pb(eb);
     std::vector<ProgramBuilder::Root> stores;
     for (size_t i = 0; i < roots.size(); ++i) stores.push_back({roots[i], ProgramBuilder::STORE, (uint32_t)i});
     if (!pb.scope(stores)) { set_error("%s: %s", what.c_str(), pb.error.c_str()); return ZKB_ERR_ARG; }
     DeviceProgram dp;
     ZKB_TRY(upload_program(pool, pb, eb, dp, st));
+    if (nregs) *nregs = dp.nregs;
     Fr **d_outs = nullptr;
     ZKB_TRY(upload_table(pool, outs, &d_outs, st));
-    return expr_run_device(pk->ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, pk->k, 1, 0, st);
+    return expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, log_n, 1, 0, st);
 }
 // out (+)= sum_i coefs[i] * polys[i] over n coefficients.  `coefs` is copied asynchronously: keep it alive until the stream is synchronised.
 static int32_t lincomb(zkb_pk *pk, DevPool &pool, const std::vector<Fr *> &polys, const std::vector<Fr> &coefs, Fr *out, bool accumulate, cudaStream_t st) {
@@ -1112,7 +1115,7 @@ static int32_t lookup_prepare(zkb_session *s, ProofState &ps) {
         roots.push_back(compress_exprs(cs, lk.table, eb, sm, s->challenges, memo, ps.theta));
         std::vector<Fr *> outs = ps.lk_f[l];
         outs.push_back(ps.lk_t[l]);
-        ZKB_TRY(run_store_program(pk, pool, eb, roots, outs, ps.d_vcols, "lookup " + std::to_string(l), st));
+        ZKB_TRY(run_store_program(pk->ctx, pk->k, pool, eb, roots, outs, ps.d_vcols, "lookup " + std::to_string(l), st));
         // multiplicities over the usable rows
         uint32_t tsize = 1;
         while (tsize < 2 * usable) tsize <<= 1;
@@ -1198,7 +1201,7 @@ static int32_t permutation_commit(zkb_session *s, ProofState &ps, const uint64_t
             first = false;
             delta_pow = fp_mul(delta_pow, delta);
         }
-        ZKB_TRY(run_store_program(pk, pool, eb, {nnum, nden}, {num, den}, ps.d_vcols, "permutation", st));
+        ZKB_TRY(run_store_program(pk->ctx, pk->k, pool, eb, {nnum, nden}, {num, den}, ps.d_vcols, "permutation", st));
         ZKB_TRY(batch_invert_device(ctx, den, tmp, n, st));
         mul_arrays_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(num, tmp, den, n);  // den <- modified values
         ctx->launches++;
@@ -1264,14 +1267,14 @@ static int32_t lookup_commit_grand_sum(zkb_session *s, ProofState &ps, const uin
                 roots.push_back(eb.add(eb.col((uint32_t)j, 0), eb.constant(ps.beta)));
                 outs.push_back(dens + j * n);
             }
-            ZKB_TRY(run_store_program(pk, pool, eb, roots, outs, d_cols, "lookup sum", st));
+            ZKB_TRY(run_store_program(pk->ctx, pk->k, pool, eb, roots, outs, d_cols, "lookup sum", st));
         }
         ZKB_TRY(batch_invert_device(ctx, dens, invs, (J + 1) * n, st));
         {
             ExprBuilder eb;
             uint32_t acc = eb.neg(eb.mul(eb.col((uint32_t)J + 1, 0), eb.col((uint32_t)(J + 2 + J), 0)));  // - m / (t + beta)
             for (size_t j = 0; j < J; ++j) acc = eb.add(acc, eb.col((uint32_t)(J + 2 + j), 0));
-            ZKB_TRY(run_store_program(pk, pool, eb, {acc}, {dterm}, d_cols, "lookup sum", st));
+            ZKB_TRY(run_store_program(pk->ctx, pk->k, pool, eb, {acc}, {dterm}, d_cols, "lookup sum", st));
         }
         ZKB_TRY(prefix_sum_device(ctx, dterm, n, Fr::zero(), ps.phis[l], st));
         ZKB_CUDA(cudaMemcpyAsync(ps.phis[l] + (n - bf), phi_blinds + 4ull * bf * l, (size_t)bf * sizeof(Fr), cudaMemcpyHostToDevice, st));
@@ -1805,5 +1808,59 @@ extern "C" int32_t zkb_prove_finish(zkb_session *s, const uint64_t *z_blinds, co
                                                      (unsigned long long)proof_cap, (unsigned long long)s->proof.size()); return ZKB_ERR_ARG; }
         memcpy(proof_out, s->proof.data(), s->proof.size());
     }
+    return ZKB_OK;
+}
+
+// ================================================================================================ C ABI: constraint interpreter
+// The gates of a CSF evaluated over caller columns by the prover's own compiler (translate, ProgramBuilder, quotient_gates) and
+// interpreter (expr_run_device): the hot kernel of a proof checked row by row against a reference evaluator.
+extern "C" int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, int32_t mode, const uint64_t *challenges,
+                                     const uint64_t y[4], const uint64_t scale[4], const uint64_t *const *columns_dev,
+                                     uint64_t *const *outs_dev, uint32_t out_stride, uint32_t out_offset, uint32_t *nregs_out, void *stream) {
+    ZKB_ARG(ctx && csf && columns_dev && outs_dev && (mode == 0 || mode == 1));
+    ZKB_ARG(mode == 0 ? out_stride == 1 && out_offset == 0 : y && scale && out_stride >= 1);
+    ZKB_CUDA(cudaSetDevice(ctx->device));
+    ZKB_TRY(zkb_csf_validate(csf, csf_words));
+    Csf cs;
+    parse_csf(csf, csf_words, cs);
+    ZKB_ARG(cs.nch == 0 || challenges);
+    std::vector<Fr> ch(cs.nch);
+    for (uint32_t i = 0; i < cs.nch; ++i) memcpy(ch[i].l, challenges + 4 * i, sizeof(Fr));
+    cudaStream_t st = pick_stream(ctx, stream);
+    const SlotMap sm(cs);
+    std::vector<Fr *> cols(cs.nf + cs.na + cs.ni);
+    for (size_t i = 0; i < cols.size(); ++i) cols[i] = (Fr *)columns_dev[i];
+    DevPool pool;
+    pool.ctx = ctx;
+    Fr **d_cols = nullptr;
+    ZKB_TRY(upload_table(pool, cols, &d_cols, st));
+    ExprBuilder eb;
+    std::vector<int64_t> memo(cs.nodes.size(), -1);
+    int nregs = 0;
+    if (mode == 0) {   // every gate one root of ONE CSE scope, like the lookup compression programs
+        std::vector<uint32_t> roots;
+        std::vector<Fr *> outs;
+        for (size_t i = 0; i < cs.gates.size(); ++i) {
+            roots.push_back(translate(cs, cs.gates[i], eb, sm, ch, memo));
+            outs.push_back((Fr *)outs_dev[i]);
+        }
+        ZKB_TRY(run_store_program(ctx, cs.k, pool, eb, roots, outs, d_cols, "gates", st, &nregs));
+    } else {           // the gate part of evaluate_h's quotient program, then one STOREACC with `scale`
+        Fr yv, sv;
+        memcpy(yv.l, y, sizeof(Fr));
+        memcpy(sv.l, scale, sizeof(Fr));
+        ProgramBuilder pb(eb);
+        const uint32_t y_idx = eb.const_slot(yv);
+        ZKB_TRY(quotient_gates(cs, ch, eb, pb, sm, memo, yv, y_idx));
+        pb.store_acc(0, eb.const_slot(sv));
+        DeviceProgram dp;
+        ZKB_TRY(upload_program(pool, pb, eb, dp, st));
+        nregs = dp.nregs;
+        Fr **d_outs = nullptr;
+        ZKB_TRY(upload_table(pool, std::vector<Fr *>{(Fr *)outs_dev[0]}, &d_outs, st));
+        ZKB_TRY(expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, cs.k, out_stride, out_offset, st));
+    }
+    ZKB_CUDA(cudaStreamSynchronize(st));   // the program buffers go back to the context's block cache on return
+    if (nregs_out) *nregs_out = (uint32_t)nregs;
     return ZKB_OK;
 }

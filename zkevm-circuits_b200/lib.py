@@ -74,6 +74,8 @@ SIGNATURES = {
     "zkb_pk_destroy": (ctypes.c_int32, [_vp]),
     "zkb_pk_vk_bytes": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, ctypes.POINTER(ctypes.c_uint64)]),
     "zkb_csf_validate": (ctypes.c_int32, [_vp, ctypes.c_uint64]),
+    "zkb_expr_eval_dev": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, ctypes.c_int32, _vp, _vp, _vp, _vp, _vp, ctypes.c_uint32,
+                                           ctypes.c_uint32, ctypes.POINTER(ctypes.c_uint32), _vp]),
     "zkb_prove_begin": (ctypes.c_int32, [_vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
     "zkb_prove_begin_ex": (ctypes.c_int32, [_vp, ctypes.c_int32, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
     "zkb_prove_begin_cb": (ctypes.c_int32, [_vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),

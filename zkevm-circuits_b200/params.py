@@ -175,9 +175,9 @@ class Srs:
         return self._commit(1, values_dev)
 
     def close(self):
-        if self.handle:
+        if self.handle and self.ctx.handle:   # not after its context: see plonk.ProvingKey.close
             self.ctx.lib.zkb_srs_destroy(self.handle)
-            self.handle = None
+        self.handle = None
 
     def __del__(self):
         try: self.close()

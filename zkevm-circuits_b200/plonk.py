@@ -107,6 +107,40 @@ def validate_csf(blob):
     check(load_library().zkb_csf_validate(_vp(b.ctypes.data), b.size))
 
 
+def expr_eval(cs, columns, mode=0, challenges=(), y=None, scale=None, out=None, out_stride=1, out_offset=0, ctx=None):
+    """The gates of `cs` evaluated by the prover's own expression compiler and interpreter (zkb_expr_eval_dev), on torch's current stream.
+
+    columns: torch int64 CUDA tensors (n, 4) in slot order fixed | advice | instance.  challenges: 4-limb Montgomery values.
+    mode 0 -> one (n, 4) tensor per gate.  mode 1 -> [out]: scale * (the gates folded in y as the quotient program folds them) at
+    rows i * out_stride + out_offset of `out` (allocated zeroed, n * out_stride rows, when None); other rows are left as they were.
+    Returns (outputs, register count of the program)."""
+    import torch
+    from .arithmetic import _cur_stream
+    ctx = ctx or default_context(columns[0].device.index)
+    n = cs.n
+    assert len(columns) == cs.num_fixed + cs.num_advice + cs.num_instance
+    assert all(c.is_cuda and c.dtype == torch.int64 and c.is_contiguous() and c.shape == (n, 4) for c in columns)
+    blob = cs.to_csf()
+    if mode == 0:
+        outs = [torch.empty((n, 4), dtype=torch.int64, device=columns[0].device) for _ in cs.gates]
+    else:
+        if out is None:
+            out = torch.zeros((n * out_stride, 4), dtype=torch.int64, device=columns[0].device)
+        assert out.is_cuda and out.dtype == torch.int64 and out.is_contiguous() and out.shape[0] > (n - 1) * out_stride + out_offset
+        outs = [out]
+    ch = np.ascontiguousarray(np.asarray(challenges, dtype=np.uint64).reshape(-1, 4))
+    yl = np.ascontiguousarray(np.asarray(y if y is not None else [0] * 4, dtype=np.uint64).reshape(4))
+    sl = np.ascontiguousarray(np.asarray(scale if scale is not None else [0] * 4, dtype=np.uint64).reshape(4))
+    ctbl = (ctypes.c_void_p * len(columns))(*[c.data_ptr() for c in columns])
+    otbl = (ctypes.c_void_p * max(1, len(outs)))(*[o.data_ptr() for o in outs])
+    nregs = ctypes.c_uint32(0)
+    check(ctx.lib.zkb_expr_eval_dev(ctx.handle, _vp(blob.ctypes.data), blob.size, int(mode), _vp(ch.ctypes.data) if ch.size else None,
+                                    _vp(yl.ctypes.data) if y is not None else None, _vp(sl.ctypes.data) if scale is not None else None,
+                                    ctypes.cast(ctbl, _vp), ctypes.cast(otbl, _vp), int(out_stride), int(out_offset), ctypes.byref(nregs),
+                                    _cur_stream()))
+    return outs, int(nregs.value)
+
+
 def _ptr_array(arrs):
     """host numpy arrays, device buffers (objects with a `device_ptr` attribute) or None -> (keepalive list, void** as c_void_p array)."""
     keep, ptrs = [], []
@@ -176,9 +210,11 @@ class ProvingKey:
         return bytes(out)
 
     def close(self):
-        if self.handle:
+        # finalisers of garbage run in no fixed order (at interpreter exit a failed test's traceback can hold the last key): once
+        # the context is destroyed the key's C state points into freed memory, so it is dropped, not destroyed
+        if self.handle and self.ctx.handle:
             self.ctx.lib.zkb_pk_destroy(self.handle)
-            self.handle = None
+        self.handle = None
 
     def __del__(self):
         try: self.close()
