@@ -51,7 +51,8 @@ ZKB_API uint32_t zkb_version(void);
 ZKB_API uint64_t zkb_launch_count(const zkb_ctx *ctx);
 ZKB_API int32_t zkb_sync(zkb_ctx *ctx);
 /* Device time per kernel class, measured with CUDA event pairs on the launching stream (off by default).  cls: 0 ntt_tile_kernel,
- * 1 msm_acc_chunk_kernel, 2 expr_kernel.  zkb_prof_read synchronises on the recorded events; reset != 0 clears the counters. */
+ * 1 msm_acc_chunk_kernel, 2 expr_kernel; the phases of zkb_check_witness_dev: 4 gate flags, 5 lookup flags (with the compression
+ * programs, which also count under 2), 6 copy flags, 7 counting and record extraction.  zkb_prof_read synchronises on the recorded events; reset != 0 clears the counters. */
 ZKB_API int32_t zkb_prof_enable(zkb_ctx *ctx, int32_t on);
 ZKB_API int32_t zkb_prof_read(zkb_ctx *ctx, int32_t cls, uint64_t *launches, double *ms, int32_t reset);
 /* Stream the context launches on (cudaStream_t as void*), for event timing by the caller. */
@@ -251,6 +252,37 @@ ZKB_API int32_t zkb_csf_validate(const uint32_t *csf, uint64_t csf_words);
 ZKB_API int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, int32_t mode, const uint64_t *challenges,
                                   const uint64_t y[4], const uint64_t scale[4], const uint64_t *const *columns_dev,
                                   uint64_t *const *outs_dev, uint32_t out_stride, uint32_t out_offset, uint32_t *nregs_out, void *stream);
+/* Witness check (halo2 MockProver::run + verify / assert_satisfied_par, without region information): which constraints of a CSF
+ * fail on caller columns, row by row, before any proof is attempted.  A failure is what the verifier would reject:
+ *   gate g          g(row) != 0 on ALL n rows (rotation r reads row (row + r) mod n): the quotient needs every gate to vanish on
+ *                   all of H, blinding rows included.  sub = 1 ("poisoned", MockProver's ConstraintPoisoned) when one of the gate's
+ *                   ADVICE queries reads a row >= usable = n - blinding_factors - 1 at that row: usually a selector that is not zero
+ *                   in the blinding rows.  Unlike MockProver the check uses the real numbers in the cells, not poison values: a gate
+ *                   that reads blinding rows but comes out numerically zero is not reported.
+ *   lookup l, set j the input tuple at a row < usable is not among the table tuples at rows < usable (the rows the prover's
+ *                   multiplicities cover).  Tuples are compared compressed with the caller's theta: a reported failure is always
+ *                   real; a real one is missed only on a theta collision, probability at most #inputs * #table rows * (width - 1) / r
+ *                   (below 2^-200 for k <= 26).  theta may be NULL only when every lookup has width 1.
+ *   copy i          v[lc][lr] != v[rc][rr] for copies_dev[i] = (lc, lr, rc, rr), columns indexing the CSF's permutation column list
+ *                   (the copy format of zkb_keygen_pk).
+ * columns_dev: HOST array of device pointers, fixed | advice | instance, 2^k elements each (instance zero-padded; advice blinded or
+ * not).  counts_out (host) receives the EXACT failure count of every gate, of every (lookup, input set) and of all copies together,
+ * in that order (n_gates + sum_l n_input_sets(l) + 1 entries), also when the records are truncated.  records_out (host) receives
+ * the first min(cap, total) failures in one fixed order: gates by (gate, row), then lookups by (lookup, set, row), then copies by
+ * index; *n_records their number; cap = 0 returns counts only.  The output is deterministic (same inputs, same bytes).
+ * Returns ZKB_OK whether or not anything fails (failures are data); ZKB_ERR_ARG for a malformed CSF, missing challenges or theta,
+ * or a copy entry out of range (column >= P or row >= n; the message names the first one).  Rank-local, also on a context with a
+ * communicator.  Temporary device memory comes from the context's block cache and is returned before the call returns.
+ * Synchronises `stream`.                                                                                                        */
+typedef struct zkb_check_record {
+    uint32_t kind;    /* 0 gate, 1 lookup, 2 copy */
+    uint32_t index;   /* gate index, lookup argument index, or position in the copy list */
+    uint32_t sub;     /* gate: poisoned (0/1); lookup: input set; copy: 0 */
+    uint32_t row;     /* the failing row; copy: the left row */
+} zkb_check_record;
+ZKB_API int32_t zkb_check_witness_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, const uint64_t *const *columns_dev,
+                                      const uint64_t *challenges, const uint64_t *theta, const uint32_t *copies_dev, uint64_t n_copies,
+                                      uint64_t *counts_out, zkb_check_record *records_out, uint32_t cap, uint32_t *n_records, void *stream);
 ZKB_API int32_t zkb_prove_begin(zkb_pk *pk, const uint64_t transcript_repr[4], const uint64_t *const *instance_values,
                                 const uint32_t *instance_lens, zkb_session **out);
 /* Same with a choice of transcript: 0 = Blake2bWrite/Challenge255 (the reference's benches, circuit-benchmarks/src/super_circuit.rs:112),

@@ -9,6 +9,10 @@ use std::os::raw::{c_char, c_void};
 #[repr(C)] pub struct zkb_pk { _p: [u8; 0] }
 #[repr(C)] pub struct zkb_session { _p: [u8; 0] }
 
+/// one failure of zkb_check_witness_dev: kind 0 gate (sub = poisoned), 1 lookup (sub = input set), 2 copy (index = copy, row = left row)
+#[repr(C)] #[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct zkb_check_record { pub kind: u32, pub index: u32, pub sub: u32, pub row: u32 }
+
 /// create_proof's generic `T: TranscriptWrite` as four C callbacks (see gpu/transcript.rs)
 #[repr(C)]
 pub struct zkb_transcript_vtable {
@@ -40,6 +44,10 @@ extern "C" {
     pub fn zkb_csf_validate(csf: *const u32, csf_words: u64) -> i32;
     pub fn zkb_keygen_pk(ctx: *mut zkb_ctx, csf: *const u32, csf_words: u64, fixed: *const *const u64, copies: *const u32, n_copies: u64,
                          srs: *mut zkb_srs, out: *mut *mut zkb_pk) -> i32;
+    // witness check (MockProver::run + assert_satisfied_par): counts per gate / lookup input set / all copies, first `cap` records
+    pub fn zkb_check_witness_dev(ctx: *mut zkb_ctx, csf: *const u32, csf_words: u64, columns_dev: *const *const u64, challenges: *const u64,
+                                 theta: *const u64, copies_dev: *const u32, n_copies: u64, counts_out: *mut u64,
+                                 records_out: *mut zkb_check_record, cap: u32, n_records: *mut u32, stream: *mut c_void) -> i32;
     pub fn zkb_pk_create_with_srs(ctx: *mut zkb_ctx, csf: *const u32, csf_words: u64, fixed: *const *const u64, sigma: *const *const u64,
                                   srs: *mut zkb_srs, out: *mut *mut zkb_pk) -> i32;
     pub fn zkb_pk_vk_bytes(pk: *mut zkb_pk, out: *mut u8, cap: u64, len: *mut u64) -> i32;

@@ -84,8 +84,8 @@ struct zkb_ctx {
     struct ProfPair { cudaEvent_t a, b; int cls; };
     std::vector<ProfPair> prof_pending;
     std::vector<cudaEvent_t> prof_free;
-    double prof_ms[4] = {0, 0, 0, 0};
-    uint64_t prof_count[4] = {0, 0, 0, 0};
+    double prof_ms[8] = {};
+    uint64_t prof_count[8] = {};
     bool ntt_ready = false;   // per-device kernel attributes / constants of ntt.cu are set (a context owns one device)
     uint64_t msm_last_adds = 0;
     uint32_t msm_last_levels = 0;   // reduction levels >= 1 the last MSM actually executed (device-side decision)
@@ -118,8 +118,10 @@ int32_t scratch_get(zkb_ctx *ctx, int slot, size_t bytes, void **out);
 int32_t block_alloc(zkb_ctx *ctx, size_t bytes, void **out, size_t *got);
 void block_free(zkb_ctx *ctx, void *p, size_t bytes);
 inline cudaStream_t pick_stream(zkb_ctx *ctx, void *stream) { return stream ? (cudaStream_t)stream : ctx->stream; }
-// kernel classes of zkb_prof_read: 0 ntt_tile_kernel, 1 msm_acc_chunk_kernel, 2 expr_kernel (quotient / lookup interpreter)
-enum ProfClass { PROF_NTT = 0, PROF_MSM_ACC = 1, PROF_EXPR = 2, PROF_OTHER = 3 };
+// kernel classes of zkb_prof_read: 0 ntt_tile_kernel, 1 msm_acc_chunk_kernel, 2 expr_kernel (quotient / lookup interpreter); 4-7 the
+// phases of zkb_check_witness_dev: gate flags, lookup flags (compression included), copy flags, count + extract
+enum ProfClass { PROF_NTT = 0, PROF_MSM_ACC = 1, PROF_EXPR = 2, PROF_OTHER = 3, PROF_CHECK_GATES = 4, PROF_CHECK_LOOKUPS = 5,
+                 PROF_CHECK_COPIES = 6, PROF_CHECK_EXTRACT = 7, PROF_CLASSES = 8 };
 struct ProfScope {   // records an event pair around the launches issued while it is alive (no-op unless profiling is on)
     zkb_ctx *ctx;
     cudaStream_t st;
@@ -207,6 +209,22 @@ struct DevPool {  // owns device allocations of a pk / session; blocks are recyc
     }
     int32_t fr(uint64_t n, Fr **out) { return alloc(n * sizeof(Fr), (void **)out); }
 };
+
+// ---- witness check (check.cu): one failure bitmap per item -- a gate, a lookup input set, or the copy list -- in report order
+struct CheckItem {
+    const uint32_t *bits;   // bit b of word w: row (or copy index) 32 w + b fails
+    uint64_t words;
+    uint32_t kind, index, sub;   // the record fields (zkb_check_record); copies take index = copy index, row = left row
+    uint64_t share, offset;      // extraction: records to write and where (filled by check_collect)
+};
+// bit i of bits[i / 32]: copy i's two cells differ.  Returns in *first_bad the first entry with a column >= P or a row >= n, or
+// UINT64_MAX; synchronises.
+int32_t copy_flags_device(zkb_ctx *ctx, DevPool &pool, const uint32_t *copies, uint64_t n_copies, const Fr *const *d_perm_cols, uint32_t P,
+                          uint32_t n, uint32_t *bits, uint64_t *first_bad, cudaStream_t st);
+// exact set-bit count of every item to counts_out, then the first `cap` set bits in item order to records_out (*n_records of them);
+// only counts and records leave the device; synchronises
+int32_t check_collect(zkb_ctx *ctx, DevPool &pool, const std::vector<CheckItem> &items, const uint32_t *copies, uint64_t *counts_out,
+                      zkb_check_record *records_out, uint32_t cap, uint32_t *n_records, cudaStream_t st);
 
 enum ScratchSlot { SCR_NTT = 0, SCR_MSM_A = 1, SCR_MSM_B = 2, SCR_MSM_C = 3, SCR_HOSTIO_A = 4, SCR_HOSTIO_B = 5, SCR_MISC = 6, SCR_MISC2 = 7, SCR_MSM_TBL = 8, SCR_COMM = 9, SCR_NTT_DESC = 10, SCR_MSM_D = 11, SCR_COMM_FLAG = 12, SCR_SHARD = 13 };
 }  // namespace zkb

@@ -74,7 +74,7 @@ void block_free(zkb_ctx *ctx, void *p, size_t bytes) {
 using namespace zkb;
 
 extern "C" const char *zkb_last_error(void) { return g_err; }
-extern "C" uint32_t zkb_version(void) { return (1u << 16) | 2u; }
+extern "C" uint32_t zkb_version(void) { return (1u << 16) | 3u; }
 
 extern "C" int32_t zkb_init(int32_t device, zkb_ctx **out) {
     ZKB_ARG(out != nullptr);
@@ -136,7 +136,7 @@ extern "C" int32_t zkb_prof_enable(zkb_ctx *ctx, int32_t on) {
     return ZKB_OK;
 }
 extern "C" int32_t zkb_prof_read(zkb_ctx *ctx, int32_t cls, uint64_t *launches, double *ms, int32_t reset) {
-    ZKB_ARG(ctx && cls >= 0 && cls < 4);
+    ZKB_ARG(ctx && cls >= 0 && cls < zkb::PROF_CLASSES);
     ZKB_CUDA(cudaSetDevice(ctx->device));
     for (auto &pp : ctx->prof_pending) {
         ZKB_CUDA(cudaEventSynchronize(pp.b));
@@ -150,7 +150,7 @@ extern "C" int32_t zkb_prof_read(zkb_ctx *ctx, int32_t cls, uint64_t *launches, 
     ctx->prof_pending.clear();
     if (launches) *launches = ctx->prof_count[cls];
     if (ms) *ms = ctx->prof_ms[cls];
-    if (reset) { for (int i = 0; i < 4; ++i) { ctx->prof_ms[i] = 0; ctx->prof_count[i] = 0; } }
+    if (reset) { for (int i = 0; i < zkb::PROF_CLASSES; ++i) { ctx->prof_ms[i] = 0; ctx->prof_count[i] = 0; } }
     return ZKB_OK;
 }
 

@@ -76,17 +76,63 @@ __global__ void __launch_bounds__(THREADS) expr_kernel(ExprLaunch L) {
     }
 }
 
-template <int NREGS, int THREADS>
-static int32_t launch_smem(const ExprLaunch &L, uint32_t n, cudaStream_t st) {
+// Flag build of the interpreter (zkb_check_witness_dev): a gate program whose roots are FLAG(gate) instructions.  FLAG sets bit
+// `row` of the gate's bitmap when the value is not zero.  A warp's 32 rows make one 32-bit word, written by that warp's lane 0
+// from __ballot_sync: every word has exactly one writer, no atomics, and the bitmap is the same on every run.  Lanes past the last
+// row (k < 5: fewer rows than a warp) evaluate row mod n and vote 0, so the whole warp reaches every ballot.  A separate kernel,
+// so the proof's expr_kernel builds are untouched.
+struct FlagLaunch {
+    const Instr *code;
+    uint32_t ncode;
+    const Fr *const *cols;
+    const Fr *consts;
+    uint32_t *bits;          // bitmap of gate g: bits + g * words
+    uint32_t words;          // (n + 31) / 32
+    uint32_t log_n;
+};
+
+template <int NREGS, int THREADS, bool SMEM>
+__global__ void __launch_bounds__(THREADS) expr_flag_kernel(FlagLaunch L) {
+    extern __shared__ uint4 expr_smem[];
+    const uint32_t n = 1u << L.log_n, mask = n - 1;
+    const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool live = tid < n;
+    const uint32_t row = tid & mask, word = tid >> 5;
+    RegFile<NREGS, THREADS, SMEM> regs(expr_smem);
+    for (uint32_t pc = 0; pc < L.ncode; ++pc) {
+        const Instr in = L.code[pc];
+        switch (in.op) {
+        case OP_LOADCOL: {
+            const int32_t rot = (int32_t)(int16_t)(in.imm >> 16);
+            const uint32_t r = (row + (uint32_t)rot) & mask;
+            regs.set(in.dst, fp_load(L.cols[in.imm & 0xffffu] + r));
+        } break;
+        case OP_LOADCONST: regs.set(in.dst, fp_load(L.consts + in.imm)); break;
+        case OP_ADD: { Fr a = regs.get(in.a), b = regs.get(in.b); regs.set(in.dst, fp_add(a, b)); } break;
+        case OP_SUB: { Fr a = regs.get(in.a), b = regs.get(in.b); regs.set(in.dst, fp_sub(a, b)); } break;
+        case OP_MUL: { Fr a = regs.get(in.a), b = regs.get(in.b); regs.set(in.dst, fp_mul(a, b)); } break;
+        case OP_NEG: { Fr a = regs.get(in.a); regs.set(in.dst, fp_neg(a)); } break;
+        case OP_FLAG: {
+            const uint32_t b = __ballot_sync(0xffffffffu, live && !regs.get(in.a).is_zero());
+            if ((threadIdx.x & 31) == 0 && word < L.words) L.bits[(size_t)in.imm * L.words + word] = b;
+        } break;
+        default: break;
+        }
+    }
+}
+
+// one launch of KERNEL with its register file in dynamic shared memory (NREGS x THREADS x 32 bytes)
+template <class Launch, int NREGS, int THREADS, void (*KERNEL)(Launch)>
+static int32_t launch_smem(const Launch &L, uint32_t n, cudaStream_t st) {
     constexpr size_t bytes = (size_t)NREGS * THREADS * 32;
     static bool attr_set[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     if (bytes > 48 * 1024 && dev < 64 && !attr_set[dev]) {
-        ZKB_CUDA(cudaFuncSetAttribute(expr_kernel<NREGS, THREADS, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+        ZKB_CUDA(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
         attr_set[dev] = true;
     }
-    expr_kernel<NREGS, THREADS, true><<<(n + THREADS - 1) / THREADS, THREADS, bytes, st>>>(L);
+    KERNEL<<<(n + THREADS - 1) / THREADS, THREADS, bytes, st>>>(L);
     return ZKB_OK;
 }
 
@@ -102,9 +148,23 @@ int32_t expr_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int n
     // quotient program (9-16 registers) is faster from shared memory: 1.00 s instead of 1.18 s of interpreter time per proof,
     // and the lower DRAM traffic lets the power-capped card hold higher clocks.  Programs of <= 16 registers therefore run from
     // shared memory (32 KB per block for <= 8 registers), larger ones from local memory.
-    if (nregs <= 8) ZKB_TRY((launch_smem<8, 128>(L, n, st)));
-    else if (nregs <= 16) ZKB_TRY((launch_smem<16, 128>(L, n, st)));
+    if (nregs <= 8) ZKB_TRY((launch_smem<ExprLaunch, 8, 128, expr_kernel<8, 128, true>>(L, n, st)));
+    else if (nregs <= 16) ZKB_TRY((launch_smem<ExprLaunch, 16, 128, expr_kernel<16, 128, true>>(L, n, st)));
     else expr_kernel<64, 128, false><<<blocks, 128, 0, st>>>(L);
+    ctx->launches++;
+    ZKB_CUDA(cudaGetLastError());
+    return ZKB_OK;
+}
+
+// the flag build over 2^log_n rows: FLAG(g) writes words [g * words, (g + 1) * words) of `bits` (device pointers as above); the
+// register bands are those of expr_run_device
+int32_t expr_flag_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int nregs, const Fr *const *d_cols, const Fr *d_consts,
+                             uint32_t *bits, uint32_t words, uint32_t log_n, cudaStream_t st) {
+    FlagLaunch L{d_code, ncode, d_cols, d_consts, bits, words, log_n};
+    const uint32_t n = 1u << log_n;
+    if (nregs <= 8) ZKB_TRY((launch_smem<FlagLaunch, 8, 128, expr_flag_kernel<8, 128, true>>(L, n, st)));
+    else if (nregs <= 16) ZKB_TRY((launch_smem<FlagLaunch, 16, 128, expr_flag_kernel<16, 128, true>>(L, n, st)));
+    else expr_flag_kernel<64, 128, false><<<(n + 127) / 128, 128, 0, st>>>(L);
     ctx->launches++;
     ZKB_CUDA(cudaGetLastError());
     return ZKB_OK;

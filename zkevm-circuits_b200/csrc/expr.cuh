@@ -31,6 +31,7 @@ enum : uint8_t {
     OP_CLEARACC = 9,
     OP_HORNER2 = 10,  // acc2 = acc2 * consts[imm] + reg[a]            (inner Horner of a run of constraints sharing one factor)
     OP_FOLD = 11,     // acc = acc * consts[imm] + reg[a] * acc2; acc2 = 0
+    OP_FLAG = 12,     // bit `row` of bitmap imm = (reg[a] != 0)     (flag build only: expr_flag_kernel, the witness check)
 };
 
 struct alignas(8) Instr {
@@ -96,7 +97,7 @@ public:
     std::string error;
 
     // evaluate `roots` (node ids) within one CSE scope and call emit_root(i, reg) after each is available
-    enum RootAction { HORNER, STORE, HORNER2, FOLD };
+    enum RootAction { HORNER, STORE, HORNER2, FOLD, FLAG };
     struct Root { uint32_t node; RootAction action; uint32_t imm; };
     bool scope(const std::vector<Root> &roots);
     void clear_acc() { code.push_back(Instr{OP_CLEARACC, 0, 0, 0, 0}); }
@@ -194,6 +195,7 @@ inline bool ProgramBuilder::scope(const std::vector<Root> &roots) {
         if (r.action == HORNER) code.push_back(Instr{OP_HORNER, 0, (uint8_t)rr, 0, r.imm});
         else if (r.action == HORNER2) code.push_back(Instr{OP_HORNER2, 0, (uint8_t)rr, 0, r.imm});
         else if (r.action == FOLD) code.push_back(Instr{OP_FOLD, 0, (uint8_t)rr, 0, r.imm});
+        else if (r.action == FLAG) code.push_back(Instr{OP_FLAG, 0, (uint8_t)rr, 0, r.imm});
         else code.push_back(Instr{OP_STORE, 0, (uint8_t)rr, 0, r.imm});
         release_use(r.node);
     }

@@ -31,6 +31,8 @@ namespace zkb {
 
 int32_t expr_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int nregs, const Fr *const *d_cols, const Fr *d_consts,
                         Fr *const *d_outs, uint32_t log_n, uint32_t out_stride, uint32_t out_offset, cudaStream_t st);
+int32_t expr_flag_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int nregs, const Fr *const *d_cols, const Fr *d_consts,
+                             uint32_t *bits, uint32_t words, uint32_t log_n, cudaStream_t st);
 
 // ---------------------------------------------------------------------------------------------------------- CSF
 enum { N_CONST = 0, N_FIXED = 1, N_ADVICE = 2, N_INSTANCE = 3, N_CHALLENGE = 4, N_NEG = 5, N_ADD = 6, N_MUL = 7, N_SCALED = 8 };
@@ -163,6 +165,25 @@ __global__ void m_count_kernel(const Fr *__restrict__ f, const Fr *__restrict__ 
     // most rows of a zkEVM lookup hit the same few table rows (selector off -> the all-zero row): aggregate per warp
     const uint32_t peers = __match_any_sync(0xffffffffu, target);
     if (target != 0xffffffffu && (threadIdx.x & 31) == (uint32_t)(__ffs(peers) - 1)) atomicAdd(&counts[target], (uint32_t)__popc(peers));
+}
+// witness check: the same probe as m_count_kernel, but one bit per row (word i / 32 by __ballot_sync, one writer per word) saying
+// "input row i < usable is not in the table"; launched over all words of the bitmap, rows >= usable vote 0
+__global__ void m_member_kernel(const Fr *__restrict__ f, const Fr *__restrict__ t, uint32_t usable, const uint32_t *__restrict__ slots,
+                                uint32_t mask, uint32_t *__restrict__ bits, uint32_t words) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    bool missing = false;
+    if (i < usable) {
+        const Fr key = fp_load(f + i);
+        uint32_t h = key_hash(key) & mask;
+        while (true) {
+            const uint32_t s = slots[h];
+            if (s == 0) { missing = true; break; }
+            if (fp_load(t + (s - 1)) == key) break;
+            h = (h + 1) & mask;
+        }
+    }
+    const uint32_t b = __ballot_sync(0xffffffffu, missing);
+    if ((threadIdx.x & 31) == 0 && (i >> 5) < words) bits[i >> 5] = b;
 }
 __global__ void counts_to_fr_kernel(const uint32_t *__restrict__ counts, uint32_t n, Fr *__restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1862,5 +1883,141 @@ extern "C" int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t
     }
     ZKB_CUDA(cudaStreamSynchronize(st));   // the program buffers go back to the context's block cache on return
     if (nregs_out) *nregs_out = (uint32_t)nregs;
+    return ZKB_OK;
+}
+
+// ================================================================================================ C ABI: witness check
+// MockProver::run + assert_satisfied on the device (semantics in zkb200.h): one bitmap per gate (the interpreter's flag build, one
+// CSE scope per gate), per lookup input set (compression as lookup_prepare computes it, the table in m_insert_kernel's hash table,
+// m_member_kernel) and for the copy list (check.cu), then exact counts and the first `cap` records (check_collect).
+extern "C" int32_t zkb_check_witness_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, const uint64_t *const *columns_dev,
+                                         const uint64_t *challenges, const uint64_t *theta, const uint32_t *copies_dev, uint64_t n_copies,
+                                         uint64_t *counts_out, zkb_check_record *records_out, uint32_t cap, uint32_t *n_records, void *stream) {
+    ZKB_ARG(ctx && csf && columns_dev && counts_out && n_records && (records_out || cap == 0) && (copies_dev || n_copies == 0));
+    ZKB_ARG(n_copies < (1ull << 32));
+    ZKB_CUDA(cudaSetDevice(ctx->device));
+    ZKB_TRY(zkb_csf_validate(csf, csf_words));
+    Csf cs;
+    parse_csf(csf, csf_words, cs);
+    if (cs.nch && !challenges) { set_error("zkb_check_witness_dev: the constraint system has %u challenges and none were given", cs.nch); return ZKB_ERR_ARG; }
+    for (size_t l = 0; l < cs.lookups.size(); ++l)
+        if (cs.lookups[l].table.size() > 1 && !theta) {
+            set_error("zkb_check_witness_dev: lookup %zu has width %zu and needs theta", l, cs.lookups[l].table.size());
+            return ZKB_ERR_ARG;
+        }
+    std::vector<Fr> ch(cs.nch);
+    for (uint32_t i = 0; i < cs.nch; ++i) memcpy(ch[i].l, challenges + 4 * i, sizeof(Fr));
+    Fr th = Fr::zero();
+    if (theta) memcpy(th.l, theta, sizeof(Fr));
+    cudaStream_t st = pick_stream(ctx, stream);
+    const uint32_t n = 1u << cs.k, words = (n + 31) / 32;
+    const uint32_t usable = n > cs.bf + 1 ? n - cs.bf - 1 : 0;
+    const SlotMap sm(cs);
+    std::vector<Fr *> cols(cs.nf + cs.na + cs.ni);
+    for (size_t i = 0; i < cols.size(); ++i) cols[i] = (Fr *)columns_dev[i];
+    size_t nsets = 0, maxsets = 0;
+    for (auto &lk : cs.lookups) { nsets += lk.inputs.size(); maxsets = std::max(maxsets, lk.inputs.size()); }
+    const uint64_t copy_words = (n_copies + 31) / 32;
+    DevPool pool;
+    pool.ctx = ctx;
+    Fr **d_cols = nullptr;
+    uint32_t *bits = nullptr;
+    ZKB_TRY(upload_table(pool, cols, &d_cols, st));
+    ZKB_TRY(pool.alloc(((cs.gates.size() + nsets) * words + copy_words) * 4, (void **)&bits));
+    uint32_t *lk_bits = bits + cs.gates.size() * words, *copy_bits = lk_bits + nsets * words;
+    std::vector<CheckItem> items;
+
+    if (!cs.gates.empty()) {   // gates: one scope per gate, no selector folding
+        ProfScope ps_(ctx, PROF_CHECK_GATES, st);
+        ExprBuilder eb;
+        ProgramBuilder pb(eb);
+        std::vector<int64_t> memo(cs.nodes.size(), -1);
+        for (size_t g = 0; g < cs.gates.size(); ++g)
+            if (!pb.scope({{translate(cs, cs.gates[g], eb, sm, ch, memo), ProgramBuilder::FLAG, (uint32_t)g}})) {
+                set_error("gate %zu: %s", g, pb.error.c_str());
+                return ZKB_ERR_ARG;
+            }
+        DeviceProgram dp;
+        ZKB_TRY(upload_program(pool, pb, eb, dp, st));
+        ZKB_TRY(expr_flag_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, bits, words, cs.k, st));
+    }
+    for (size_t g = 0; g < cs.gates.size(); ++g) items.push_back({bits + g * words, words, 0, (uint32_t)g, 0, 0, 0});
+
+    if (nsets) {               // lookups, one argument at a time: compressed inputs and table, the table's hash set, membership bits
+        ProfScope ps_(ctx, PROF_CHECK_LOOKUPS, st);
+        std::vector<Fr *> bufs(maxsets + 1);
+        for (auto &b : bufs) ZKB_TRY(pool.fr(n, &b));
+        uint32_t tsize = 1;
+        while (tsize < 2 * usable) tsize <<= 1;
+        uint32_t *slots = nullptr;
+        ZKB_TRY(pool.alloc((size_t)tsize * 4, (void **)&slots));
+        uint32_t *out = lk_bits;
+        for (size_t l = 0; l < cs.lookups.size(); ++l) {
+            const CsfLookup &lk = cs.lookups[l];
+            const size_t ns = lk.inputs.size();
+            ExprBuilder eb;
+            std::vector<int64_t> memo(cs.nodes.size(), -1);
+            std::vector<uint32_t> roots;
+            for (size_t j = 0; j < ns; ++j) roots.push_back(compress_exprs(cs, lk.inputs[j], eb, sm, ch, memo, th));
+            roots.push_back(compress_exprs(cs, lk.table, eb, sm, ch, memo, th));
+            std::vector<Fr *> outs(bufs.begin(), bufs.begin() + ns);
+            outs.push_back(bufs[maxsets]);
+            ZKB_TRY(run_store_program(ctx, cs.k, pool, eb, roots, outs, d_cols, "lookup " + std::to_string(l), st));
+            ZKB_CUDA(cudaMemsetAsync(slots, 0, (size_t)tsize * 4, st));
+            if (usable) {
+                m_insert_kernel<<<(usable + 255) / 256, 256, 0, st>>>(bufs[maxsets], usable, slots, tsize - 1);
+                ctx->launches++;
+            }
+            for (size_t j = 0; j < ns; ++j, out += words) {
+                m_member_kernel<<<(n + 255) / 256, 256, 0, st>>>(bufs[j], bufs[maxsets], usable, slots, tsize - 1, out, words);
+                ctx->launches++;
+                items.push_back({out, words, 1, (uint32_t)l, (uint32_t)j, 0, 0});
+            }
+            ZKB_CUDA(cudaGetLastError());
+        }
+    }
+
+    {                          // copies
+        ProfScope ps_(ctx, PROF_CHECK_COPIES, st);
+        std::vector<Fr *> pc;
+        for (auto &c : cs.perm) pc.push_back(cols[sm.perm(c)]);
+        Fr **d_pc = nullptr;
+        ZKB_TRY(upload_table(pool, pc, &d_pc, st));
+        uint64_t first_bad = 0;
+        ZKB_TRY(copy_flags_device(ctx, pool, copies_dev, n_copies, d_pc, (uint32_t)pc.size(), n, copy_bits, &first_bad, st));
+        if (first_bad != ~0ull) {
+            set_error("zkb_check_witness_dev: copy constraint %llu is out of range (column >= %zu or row >= %u)", (unsigned long long)first_bad,
+                      pc.size(), n);
+            return ZKB_ERR_ARG;
+        }
+    }
+    items.push_back({copy_bits, copy_words, 2, 0, 0, 0, 0});
+
+    ZKB_TRY(check_collect(ctx, pool, items, copies_dev, counts_out, records_out, cap, n_records, st));
+    // poisoned gate failures: an advice query of the gate reads a row >= usable at the failing row
+    std::vector<std::vector<int32_t>> adv_rots(cs.gates.size());
+    std::vector<bool> adv_rots_done(cs.gates.size(), false);
+    for (uint32_t i = 0; i < *n_records && records_out[i].kind == 0; ++i) {
+        zkb_check_record &r = records_out[i];
+        std::vector<int32_t> &rots = adv_rots[r.index];
+        if (!adv_rots_done[r.index]) {
+            std::vector<uint32_t> stack{cs.gates[r.index]};
+            std::vector<bool> seen(cs.nodes.size(), false);
+            while (!stack.empty()) {
+                const uint32_t v = stack.back();
+                stack.pop_back();
+                if (seen[v]) continue;
+                seen[v] = true;
+                const auto &nd = cs.nodes[v];
+                if (nd[0] == N_ADVICE) rots.push_back((int32_t)nd[2]);
+                else if (nd[0] == N_NEG || nd[0] == N_SCALED) stack.push_back(nd[1]);
+                else if (nd[0] == N_ADD || nd[0] == N_MUL) { stack.push_back(nd[1]); stack.push_back(nd[2]); }
+            }
+            adv_rots_done[r.index] = true;
+        }
+        r.sub = 0;
+        for (int32_t rot : rots)
+            if (((r.row + (uint32_t)rot) & (n - 1)) >= usable) { r.sub = 1; break; }
+    }
     return ZKB_OK;
 }

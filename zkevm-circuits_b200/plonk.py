@@ -8,9 +8,11 @@ Nothing in this module computes field arithmetic on the CPU; it only marshals bu
 """
 import ctypes
 import struct
+from collections import namedtuple
+
 import numpy as np
 
-from .lib import check, default_context
+from .lib import ZkbError, check, default_context
 
 _vp = ctypes.c_void_p
 CONST, FIXED, ADVICE, INSTANCE, CHALLENGE, NEG, ADD, MUL, SCALED = range(9)
@@ -139,6 +141,117 @@ def expr_eval(cs, columns, mode=0, challenges=(), y=None, scale=None, out=None, 
                                     ctypes.cast(ctbl, _vp), ctypes.cast(otbl, _vp), int(out_stride), int(out_offset), ctypes.byref(nregs),
                                     _cur_stream()))
     return outs, int(nregs.value)
+
+
+R_MOD = 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001
+GATE, LOOKUP, COPY = 0, 1, 2
+Failure = namedtuple("Failure", "kind index sub row")   # zkb_check_record: sub = poisoned (gate) / input set (lookup) / 0 (copy)
+
+
+class _CheckRecord(ctypes.Structure):
+    _fields_ = [("kind", ctypes.c_uint32), ("index", ctypes.c_uint32), ("sub", ctypes.c_uint32), ("row", ctypes.c_uint32)]
+
+
+class WitnessReport:
+    """What check_witness found: `counts` holds the exact failure count of every gate, every (lookup, input set) and of all copies
+    together, in that order (also as `gate_counts`, `lookup_counts` {(lookup, set): count} and `copy_count`); `failures` holds the
+    first `cap` failures as Failure tuples, gates by (gate, row), then lookups by (lookup, set, row), then copies by index."""
+
+    def __init__(self, cs, counts, failures, copies):
+        self.counts = counts
+        self.failures = failures
+        self._copies = copies
+        ng = len(cs.gates)
+        self.gate_counts = [int(c) for c in counts[:ng]]
+        keys = [(l, j) for l, (inputs, _) in enumerate(cs.lookups) for j in range(len(inputs))]
+        self.lookup_counts = {key: int(c) for key, c in zip(keys, counts[ng:ng + len(keys)])}
+        self.copy_count = int(counts[-1])
+        self.total = int(counts.sum())
+        self.ok = self.total == 0
+
+    def __repr__(self):
+        return f"WitnessReport(ok={self.ok}, total={self.total}, records={len(self.failures)})"
+
+    def summary(self, rows_shown=8):
+        """one line per failing item, e.g. 'gate 17 not satisfied at rows 5, 6 (and 1021 more)'"""
+        by_item = {}
+        for f in self.failures:
+            by_item.setdefault((f.kind, f.index, f.sub if f.kind == LOOKUP else 0), []).append(f)
+        lines = []
+
+        def rows_text(fs, count):
+            shown = [str(f.row) for f in fs[:rows_shown]]
+            if not shown:
+                return f"at {count} rows (not listed: the record cap was reached)"
+            more = count - len(shown)
+            return f"at row{'s' if len(shown) > 1 else ''} {', '.join(shown)}" + (f" (and {more} more)" if more else "")
+        for g, c in enumerate(self.gate_counts):
+            if c:
+                fs = by_item.get((GATE, g, 0), [])
+                poisoned = sum(f.sub for f in fs)
+                lines.append(f"gate {g} not satisfied {rows_text(fs, c)}" + (f"; {poisoned} listed rows read blinding rows (poisoned)" if poisoned else ""))
+        for (l, j), c in self.lookup_counts.items():
+            if c:
+                lines.append(f"lookup {l} set {j} {rows_text(by_item.get((LOOKUP, l, j), []), c)}")
+        copy_fs = [f for f in self.failures if f.kind == COPY]
+        for f in copy_fs[:rows_shown]:
+            lc, lr, rc, rr = (int(x) for x in self._copies(f.index))
+            lines.append(f"copy {f.index}: (col {lc}, row {lr}) != (col {rc}, row {rr})")
+        if self.copy_count > min(len(copy_fs), rows_shown):
+            lines.append(f"(and {self.copy_count - min(len(copy_fs), rows_shown)} more copy failures)")
+        return lines
+
+    def assert_satisfied(self):
+        """raise ZkbError with a readable summary unless every constraint holds (MockProver::assert_satisfied)"""
+        if not self.ok:
+            raise ZkbError(f"witness does not satisfy the constraint system ({self.total} failures):\n  " + "\n  ".join(self.summary()))
+
+
+def check_witness(cs, fixed, advice, instances, challenges=(), copies=(), theta=None, cap=1024, ctx=None):
+    """MockProver::run + verify on the GPU (zkb_check_witness_dev): which gates, lookups and copy constraints of `cs` fail on this
+    witness, by row.  fixed / advice: one column per entry, n rows each, numpy uint64 (n, 4) Montgomery arrays or int64 CUDA tensors;
+    instances: columns of at most n cells (zero-padded here).  challenges: the 4-limb values used for synthesis.  copies: (left perm
+    column, left row, right perm column, right row) entries -- columns index cs.perm_columns as for ProvingKey(copies=...) -- or an
+    int32 CUDA tensor of shape (m, 4).  theta: the lookup compression challenge (4 Montgomery limbs); None draws a fresh random one.
+    Runs on torch's current stream of the columns' device; returns a WitnessReport with at most `cap` failure records."""
+    import os
+    import torch
+    from .arithmetic import _cur_stream
+    n = cs.n
+    cols = list(fixed) + list(advice) + list(instances)
+    devs = [c.device for c in cols if isinstance(c, torch.Tensor) and c.is_cuda]
+    device = devs[0] if devs else torch.device("cuda", torch.cuda.current_device())
+    ctx = ctx or default_context(device.index)
+    assert len(fixed) == cs.num_fixed and len(advice) == cs.num_advice and len(instances) == cs.num_instance
+
+    def dev_col(c, pad=False):
+        t = c if isinstance(c, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(c, dtype=np.uint64).view(np.int64))
+        t = t.to(device=device, dtype=torch.int64).reshape(-1, 4)
+        if pad and t.shape[0] < n:
+            t = torch.cat([t, torch.zeros((n - t.shape[0], 4), dtype=torch.int64, device=device)])
+        assert t.shape == (n, 4), f"a column has {t.shape[0]} rows, expected {n}"
+        return t.contiguous()
+    dcols = [dev_col(c) for c in list(fixed) + list(advice)] + [dev_col(c, pad=True) for c in instances]
+    if isinstance(copies, torch.Tensor):
+        cp = copies.to(device=device, dtype=torch.int32).reshape(-1, 4).contiguous()
+    else:
+        cp = torch.from_numpy(np.ascontiguousarray(np.asarray(copies, dtype=np.uint32).reshape(-1, 4)).view(np.int32)).to(device)
+    if theta is None:
+        th = int.from_bytes(os.urandom(40), "little") % R_MOD   # a uniform reduced value is the Montgomery form of a uniform element
+        theta = [(th >> (64 * i)) & 0xFFFFFFFFFFFFFFFF for i in range(4)]
+    th = np.ascontiguousarray(np.asarray(theta, dtype=np.uint64).reshape(4))
+    ch = np.ascontiguousarray(np.asarray(challenges, dtype=np.uint64).reshape(-1, 4))
+    blob = cs.to_csf()
+    n_items = len(cs.gates) + sum(len(inputs) for inputs, _ in cs.lookups) + 1
+    counts = np.zeros(n_items, dtype=np.uint64)
+    recs = (_CheckRecord * max(1, cap))()
+    n_rec = ctypes.c_uint32(0)
+    ctbl = (ctypes.c_void_p * max(1, len(dcols)))(*[c.data_ptr() for c in dcols])
+    check(ctx.lib.zkb_check_witness_dev(ctx.handle, _vp(blob.ctypes.data), blob.size, ctypes.cast(ctbl, _vp),
+                                        _vp(ch.ctypes.data) if ch.size else None, _vp(th.ctypes.data), _vp(cp.data_ptr()) if cp.shape[0] else None,
+                                        cp.shape[0], _vp(counts.ctypes.data), ctypes.cast(recs, _vp), int(cap), ctypes.byref(n_rec), _cur_stream()))
+    failures = [Failure(r.kind, r.index, r.sub, r.row) for r in recs[: n_rec.value]]
+    return WitnessReport(cs, counts, failures, lambda i: cp[i].cpu().numpy().view(np.uint32))
 
 
 def _ptr_array(arrs):
