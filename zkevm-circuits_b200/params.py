@@ -174,6 +174,17 @@ class Srs:
     def commit_lagrange(self, values_dev):
         return self._commit(1, values_dev)
 
+    def commit_batch(self, basis, cols_dev):
+        """zkb_srs_commit_batch_dev: several device columns of equal length against basis 0 = g / 1 = g_lagrange, in passes of
+        msm_max_batch columns (how the prover commits a phase) -> uint64 (len(cols_dev), 8) affine points."""
+        import ctypes
+        from .lib import check
+        ptrs = (ctypes.c_void_p * len(cols_dev))(*[c.data_ptr() for c in cols_dev])
+        out = np.zeros((len(cols_dev), 8), dtype=np.uint64)
+        check(self.ctx.lib.zkb_srs_commit_batch_dev(self.handle, int(basis), ctypes.cast(ptrs, ctypes.c_void_p), len(cols_dev), cols_dev[0].shape[0],
+                                                    ctypes.c_void_p(out.ctypes.data), A._cur_stream()))
+        return out
+
     def close(self):
         if self.handle and self.ctx.handle:   # not after its context: see plonk.ProvingKey.close
             self.ctx.lib.zkb_srs_destroy(self.handle)
