@@ -252,6 +252,12 @@ ZKB_API int32_t zkb_csf_validate(const uint32_t *csf, uint64_t csf_words);
 ZKB_API int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, int32_t mode, const uint64_t *challenges,
                                   const uint64_t y[4], const uint64_t scale[4], const uint64_t *const *columns_dev,
                                   uint64_t *const *outs_dev, uint32_t out_stride, uint32_t out_offset, uint32_t *nregs_out, void *stream);
+/* Host only (no CUDA device needed): the interpreter program zkb_expr_eval_dev would run for the same csf / mode / challenges /
+ * y / scale, after operand fusion.  One 64-bit word per instruction (the Instr layout of csrc/expr.cuh: op, dst, a, b bytes,
+ * then the 32-bit imm); the first min(cap, *ncode_out) words go to code_out (may be NULL when cap is 0).  *nregs_out (may be
+ * NULL) receives the register count that picks the kernel build.  For instruction counts (scripts/expr_program_stats.py).    */
+ZKB_API int32_t zkb_expr_program(const uint32_t *csf, uint64_t csf_words, int32_t mode, const uint64_t *challenges, const uint64_t y[4],
+                                 const uint64_t scale[4], uint64_t *code_out, uint64_t cap, uint64_t *ncode_out, uint32_t *nregs_out);
 /* Witness check (halo2 MockProver::run + verify / assert_satisfied_par, without region information): which constraints of a CSF
  * fail on caller columns, row by row, before any proof is attempted.  A failure is what the verifier would reject:
  *   gate g          g(row) != 0 on ALL n rows (rotation r reads row (row + r) mod n): the quotient needs every gate to vanish on

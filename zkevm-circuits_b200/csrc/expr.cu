@@ -1,4 +1,5 @@
 // expr.cu -- device interpreter for constraint-expression programs (see expr.cuh).
+#include <type_traits>
 #include "common.cuh"
 #include "expr.cuh"
 
@@ -39,48 +40,11 @@ struct RegFile {
     }
 };
 
-template <int NREGS, int THREADS, bool SMEM>
-__global__ void __launch_bounds__(THREADS) expr_kernel(ExprLaunch L) {
-    extern __shared__ uint4 expr_smem[];
-    const uint32_t n = 1u << L.log_n, mask = n - 1;
-    const uint32_t row = blockIdx.x * blockDim.x + threadIdx.x;
-    if (row >= n) return;
-    RegFile<NREGS, THREADS, SMEM> regs(expr_smem);
-    Fr acc = Fr::zero(), acc2 = Fr::zero();
-    for (uint32_t pc = 0; pc < L.ncode; ++pc) {
-        const Instr in = L.code[pc];
-        switch (in.op) {
-        case OP_LOADCOL: {
-            const int32_t rot = (int32_t)(int16_t)(in.imm >> 16);
-            const uint32_t r = (row + (uint32_t)rot) & mask;
-            regs.set(in.dst, fp_load(L.cols[in.imm & 0xffffu] + r));
-        } break;
-        case OP_LOADCONST: regs.set(in.dst, fp_load(L.consts + in.imm)); break;
-        case OP_ADD: { Fr a = regs.get(in.a), b = regs.get(in.b); regs.set(in.dst, fp_add(a, b)); } break;
-        case OP_SUB: { Fr a = regs.get(in.a), b = regs.get(in.b); regs.set(in.dst, fp_sub(a, b)); } break;
-        case OP_MUL: { Fr a = regs.get(in.a), b = regs.get(in.b); regs.set(in.dst, fp_mul(a, b)); } break;
-        case OP_NEG: { Fr a = regs.get(in.a); regs.set(in.dst, fp_neg(a)); } break;
-        case OP_HORNER: acc = fp_add(fp_mul(acc, fp_load(L.consts + in.imm)), regs.get(in.a)); break;
-        case OP_STORE: fp_store(L.outs[in.imm] + (size_t)row * L.out_stride + L.out_offset, regs.get(in.a)); break;
-        case OP_STOREACC:
-            fp_store(L.outs[in.imm & 0xffu] + (size_t)row * L.out_stride + L.out_offset, fp_mul(acc, fp_load(L.consts + (in.imm >> 8))));
-            break;
-        case OP_CLEARACC: acc = Fr::zero(); break;
-        case OP_HORNER2: acc2 = fp_add(fp_mul(acc2, fp_load(L.consts + in.imm)), regs.get(in.a)); break;
-        case OP_FOLD:
-            acc = fp_add(fp_mul(acc, fp_load(L.consts + in.imm)), fp_mul(regs.get(in.a), acc2));
-            acc2 = Fr::zero();
-            break;
-        default: break;
-        }
-    }
-}
-
 // Flag build of the interpreter (zkb_check_witness_dev): a gate program whose roots are FLAG(gate) instructions.  FLAG sets bit
 // `row` of the gate's bitmap when the value is not zero.  A warp's 32 rows make one 32-bit word, written by that warp's lane 0
 // from __ballot_sync: every word has exactly one writer, no atomics, and the bitmap is the same on every run.  Lanes past the last
-// row (k < 5: fewer rows than a warp) evaluate row mod n and vote 0, so the whole warp reaches every ballot.  A separate kernel,
-// so the proof's expr_kernel builds are untouched.
+// row (k < 5: fewer rows than a warp) evaluate row mod n and vote 0, so the whole warp reaches every ballot.  A separate kernel
+// (the accumulator and output roots compile out of it), sharing run_program with expr_kernel.
 struct FlagLaunch {
     const Instr *code;
     uint32_t ncode;
@@ -91,34 +55,97 @@ struct FlagLaunch {
     uint32_t log_n;
 };
 
+// The interpreter loop of both kernels for thread `tid` (row tid mod n).  Every form of one operation ends in the same field
+// operation (the goto targets after the switch), so a fused form costs its operand fetches and no second copy of the arithmetic.
+template <int NREGS, int THREADS, bool SMEM, class Launch>
+__device__ __forceinline__ void run_program(const Launch &L, uint32_t tid) {
+    constexpr bool FLAG = std::is_same<Launch, FlagLaunch>::value;
+    extern __shared__ uint4 expr_smem[];
+    const uint32_t mask = (1u << L.log_n) - 1, row = tid & mask;
+    RegFile<NREGS, THREADS, SMEM> regs(expr_smem);
+    Fr acc = Fr::zero(), acc2 = Fr::zero();
+    uint32_t pc = 0;
+    auto col = [&](uint32_t imm) {   // imm = slot | rotation << 16
+        const int32_t rot = (int32_t)(int16_t)(imm >> 16);
+        return fp_load(L.cols[imm & 0xffffu] + ((row + (uint32_t)rot) & mask));
+    };
+    auto cst = [&](uint32_t i) { return fp_load(L.consts + i); };
+    auto arg = [&]() { return L.code[++pc].imm; };   // the OP_ARG word after the current instruction
+    for (; pc < L.ncode; ++pc) {
+        const Instr in = L.code[pc];
+        Fr x, y;
+        switch (in.op) {
+        case OP_LOADCOL: regs.set(in.dst, col(in.imm)); continue;
+        case OP_LOADCONST: regs.set(in.dst, cst(in.imm)); continue;
+        case OP_ADD: x = regs.get(in.a); y = regs.get(in.b); goto add;
+        case OP_ADD_RC + FORM_RC: x = regs.get(in.a); y = col(in.imm); goto add;
+        case OP_ADD_RC + FORM_CR: x = col(in.imm); y = regs.get(in.a); goto add;
+        case OP_ADD_RC + FORM_RK: x = regs.get(in.a); y = cst(in.imm); goto add;
+        case OP_ADD_RC + FORM_KR: x = cst(in.imm); y = regs.get(in.a); goto add;
+        case OP_ADD_RC + FORM_CC: x = col(in.imm); y = col(arg()); goto add;
+        case OP_ADD_RC + FORM_CK: x = col(in.imm); y = cst(arg()); goto add;
+        case OP_ADD_RC + FORM_KC: x = cst(in.imm); y = col(arg()); goto add;
+        case OP_SUB: x = regs.get(in.a); y = regs.get(in.b); goto sub;
+        case OP_SUB_RC + FORM_RC: x = regs.get(in.a); y = col(in.imm); goto sub;
+        case OP_SUB_RC + FORM_CR: x = col(in.imm); y = regs.get(in.a); goto sub;
+        case OP_SUB_RC + FORM_RK: x = regs.get(in.a); y = cst(in.imm); goto sub;
+        case OP_SUB_RC + FORM_KR: x = cst(in.imm); y = regs.get(in.a); goto sub;
+        case OP_SUB_RC + FORM_CC: x = col(in.imm); y = col(arg()); goto sub;
+        case OP_SUB_RC + FORM_CK: x = col(in.imm); y = cst(arg()); goto sub;
+        case OP_SUB_RC + FORM_KC: x = cst(in.imm); y = col(arg()); goto sub;
+        case OP_MUL: x = regs.get(in.a); y = regs.get(in.b); goto mul;
+        case OP_MUL_RC + FORM_RC: x = regs.get(in.a); y = col(in.imm); goto mul;
+        case OP_MUL_RC + FORM_CR: x = col(in.imm); y = regs.get(in.a); goto mul;
+        case OP_MUL_RC + FORM_RK: x = regs.get(in.a); y = cst(in.imm); goto mul;
+        case OP_MUL_RC + FORM_KR: x = cst(in.imm); y = regs.get(in.a); goto mul;
+        case OP_MUL_RC + FORM_CC: x = col(in.imm); y = col(arg()); goto mul;
+        case OP_MUL_RC + FORM_CK: x = col(in.imm); y = cst(arg()); goto mul;
+        case OP_MUL_RC + FORM_KC: x = cst(in.imm); y = col(arg()); goto mul;
+        case OP_NEG: regs.set(in.dst, fp_neg(regs.get(in.a))); continue;
+        case OP_FLAG:
+            if constexpr (FLAG) {
+                const uint32_t b = __ballot_sync(0xffffffffu, tid < (1u << L.log_n) && !regs.get(in.a).is_zero());
+                const uint32_t word = tid >> 5;
+                if ((threadIdx.x & 31) == 0 && word < L.words) L.bits[(size_t)in.imm * L.words + word] = b;
+            }
+            continue;
+        case OP_HORNER: case OP_HORNER_C:
+            if constexpr (!FLAG) acc = fp_add(fp_mul(acc, cst(in.imm)), in.op == OP_HORNER ? regs.get(in.a) : col(arg()));
+            continue;
+        case OP_HORNER2: case OP_HORNER2_C:
+            if constexpr (!FLAG) acc2 = fp_add(fp_mul(acc2, cst(in.imm)), in.op == OP_HORNER2 ? regs.get(in.a) : col(arg()));
+            continue;
+        case OP_FOLD: case OP_FOLD_C:
+            if constexpr (!FLAG) {
+                acc = fp_add(fp_mul(acc, cst(in.imm)), fp_mul(in.op == OP_FOLD ? regs.get(in.a) : col(arg()), acc2));
+                acc2 = Fr::zero();
+            }
+            continue;
+        case OP_STORE:
+            if constexpr (!FLAG) fp_store(L.outs[in.imm] + (size_t)row * L.out_stride + L.out_offset, regs.get(in.a));
+            continue;
+        case OP_STOREACC:
+            if constexpr (!FLAG) fp_store(L.outs[in.imm & 0xffu] + (size_t)row * L.out_stride + L.out_offset, fp_mul(acc, cst(in.imm >> 8)));
+            continue;
+        case OP_CLEARACC: acc = Fr::zero(); continue;
+        default: continue;
+        }
+    add: regs.set(in.dst, fp_add(x, y)); continue;
+    sub: regs.set(in.dst, fp_sub(x, y)); continue;
+    mul: regs.set(in.dst, fp_mul(x, y));
+    }
+}
+
+template <int NREGS, int THREADS, bool SMEM>
+__global__ void __launch_bounds__(THREADS) expr_kernel(ExprLaunch L) {
+    const uint32_t row = blockIdx.x * blockDim.x + threadIdx.x;
+    if (row >= (1u << L.log_n)) return;
+    run_program<NREGS, THREADS, SMEM>(L, row);
+}
+
 template <int NREGS, int THREADS, bool SMEM>
 __global__ void __launch_bounds__(THREADS) expr_flag_kernel(FlagLaunch L) {
-    extern __shared__ uint4 expr_smem[];
-    const uint32_t n = 1u << L.log_n, mask = n - 1;
-    const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
-    const bool live = tid < n;
-    const uint32_t row = tid & mask, word = tid >> 5;
-    RegFile<NREGS, THREADS, SMEM> regs(expr_smem);
-    for (uint32_t pc = 0; pc < L.ncode; ++pc) {
-        const Instr in = L.code[pc];
-        switch (in.op) {
-        case OP_LOADCOL: {
-            const int32_t rot = (int32_t)(int16_t)(in.imm >> 16);
-            const uint32_t r = (row + (uint32_t)rot) & mask;
-            regs.set(in.dst, fp_load(L.cols[in.imm & 0xffffu] + r));
-        } break;
-        case OP_LOADCONST: regs.set(in.dst, fp_load(L.consts + in.imm)); break;
-        case OP_ADD: { Fr a = regs.get(in.a), b = regs.get(in.b); regs.set(in.dst, fp_add(a, b)); } break;
-        case OP_SUB: { Fr a = regs.get(in.a), b = regs.get(in.b); regs.set(in.dst, fp_sub(a, b)); } break;
-        case OP_MUL: { Fr a = regs.get(in.a), b = regs.get(in.b); regs.set(in.dst, fp_mul(a, b)); } break;
-        case OP_NEG: { Fr a = regs.get(in.a); regs.set(in.dst, fp_neg(a)); } break;
-        case OP_FLAG: {
-            const uint32_t b = __ballot_sync(0xffffffffu, live && !regs.get(in.a).is_zero());
-            if ((threadIdx.x & 31) == 0 && word < L.words) L.bits[(size_t)in.imm * L.words + word] = b;
-        } break;
-        default: break;
-        }
-    }
+    run_program<NREGS, THREADS, SMEM>(L, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 // one launch of KERNEL with its register file in dynamic shared memory (NREGS x THREADS x 32 bytes)

@@ -10,6 +10,7 @@
 // theta on the Lagrange domain (mv_lookup/prover.rs `prepare`).
 #pragma once
 #include <stdint.h>
+#include <array>
 #include <map>
 #include <string>
 #include <tuple>
@@ -32,6 +33,17 @@ enum : uint8_t {
     OP_HORNER2 = 10,  // acc2 = acc2 * consts[imm] + reg[a]            (inner Horner of a run of constraints sharing one factor)
     OP_FOLD = 11,     // acc = acc * consts[imm] + reg[a] * acc2; acc2 = 0
     OP_FLAG = 12,     // bit `row` of bitmap imm = (reg[a] != 0)     (flag build only: expr_flag_kernel, the witness check)
+    OP_ARG = 13,      // not an instruction: the second 32-bit operand of the fused instruction before it
+    // Fused operand forms (ProgramBuilder::fuse).  An operand is R = reg[a], C = a column at a rotation (encoded as OP_LOADCOL's
+    // imm) or K = consts[index].  The first C / K operand is `imm`, a second one is the imm of the OP_ARG word that follows;
+    // OP_ADD_RC + form, OP_SUB_RC + form, OP_MUL_RC + form compute  left op right  for the forms below, in that order.
+    FORM_RC = 0, FORM_CR = 1, FORM_RK = 2, FORM_KR = 3, FORM_CC = 4, FORM_CK = 5, FORM_KC = 6,
+    OP_ADD_RC = 16,
+    OP_SUB_RC = 24,
+    OP_MUL_RC = 32,
+    OP_HORNER_C = 40,   // OP_HORNER / OP_HORNER2 / OP_FOLD with the term a column: consts[imm] as before, the column in OP_ARG
+    OP_HORNER2_C = 41,
+    OP_FOLD_C = 42,
 };
 
 struct alignas(8) Instr {
@@ -107,9 +119,74 @@ public:
 
 private:
     ExprBuilder &eb;
+    void fuse(size_t begin);
 };
 
+// Peephole pass over the code of one scope, code[begin..): an OP_LOADCOL / OP_LOADCONST whose register is read exactly once
+// before it is written again, by an ADD / SUB / MUL or (a column only) by a HORNER / HORNER2 / FOLD root, becomes an operand of
+// that reader, so the value goes from global memory straight into the field operation instead of through the register file.
+// Operand order, and with it every result bit, is unchanged; registers are only dropped, so max_regs_used (which picks the
+// kernel build) is the allocator's count as before.  Two constants into one instruction (no KK form): the right one stays a load.
+inline void ProgramBuilder::fuse(size_t begin) {
+    auto is_arith = [](uint8_t op) { return op == OP_ADD || op == OP_SUB || op == OP_MUL; };
+    auto is_root = [](uint8_t op) { return op == OP_HORNER || op == OP_HORNER2 || op == OP_FOLD; };
+    auto is_load = [](uint8_t op) { return op == OP_LOADCOL || op == OP_LOADCONST; };
+    auto reads = [&](const Instr &in, int s) {   // does operand slot s (0: a, 1: b) of `in` read a register
+        if (is_arith(in.op)) return true;
+        return s == 0 && (in.op == OP_NEG || is_root(in.op) || in.op == OP_STORE || in.op == OP_FLAG);
+    };
+    auto writes = [&](const Instr &in) { return is_load(in.op) || is_arith(in.op) || in.op == OP_NEG; };
+    const size_t end = code.size();
+    std::vector<std::array<int64_t, 2>> src(end - begin, {-1, -1});   // the load feeding operand slot 0 / 1, or -1
+    for (size_t i = begin; i < end; ++i) {
+        if (!is_load(code[i].op)) continue;
+        const uint8_t r = code[i].dst;
+        int uses = 0, slot = -1;
+        size_t user = 0;
+        for (size_t j = i + 1; j < end && uses < 2; ++j) {
+            for (int s = 0; s < 2; ++s)
+                if (reads(code[j], s) && (s == 0 ? code[j].a : code[j].b) == r) { ++uses; user = j; slot = s; }
+            if (writes(code[j]) && code[j].dst == r) break;
+        }
+        if (uses != 1) continue;
+        const uint8_t op = code[user].op;
+        if (is_arith(op) || (is_root(op) && code[i].op == OP_LOADCOL)) src[user - begin][slot] = (int64_t)i;
+    }
+    auto kind = [&](const std::array<int64_t, 2> &s, int k) { return s[k] < 0 ? 'R' : code[s[k]].op == OP_LOADCOL ? 'C' : 'K'; };
+    std::vector<bool> fused(end - begin, false);
+    for (auto &s : src) {
+        if (kind(s, 0) == 'K' && kind(s, 1) == 'K') s[1] = -1;
+        for (int k = 0; k < 2; ++k)
+            if (s[k] >= 0) fused[s[k] - begin] = true;
+    }
+    std::vector<Instr> out;
+    for (size_t i = begin; i < end; ++i) {
+        const Instr in = code[i];
+        const auto &s = src[i - begin];
+        if (fused[i - begin]) continue;
+        if (s[0] < 0 && s[1] < 0) { out.push_back(in); continue; }
+        if (is_root(in.op)) {
+            const uint8_t op = in.op == OP_HORNER ? OP_HORNER_C : in.op == OP_HORNER2 ? OP_HORNER2_C : OP_FOLD_C;
+            out.push_back(Instr{op, 0, 0, 0, in.imm});
+            out.push_back(Instr{OP_ARG, 0, 0, 0, code[s[0]].imm});
+            continue;
+        }
+        const char ka = kind(s, 0), kb = kind(s, 1);
+        const int form = ka == 'R' ? (kb == 'C' ? FORM_RC : FORM_RK)
+                       : kb == 'R' ? (ka == 'C' ? FORM_CR : FORM_KR)
+                       : ka == 'C' ? (kb == 'C' ? FORM_CC : FORM_CK) : FORM_KC;
+        const uint8_t base = in.op == OP_ADD ? OP_ADD_RC : in.op == OP_SUB ? OP_SUB_RC : OP_MUL_RC;
+        const int first = s[0] >= 0 ? 0 : 1;   // the first non-register operand goes to imm, a second one to OP_ARG
+        const uint8_t reg = ka == 'R' ? in.a : in.b;
+        out.push_back(Instr{(uint8_t)(base + form), in.dst, (uint8_t)(form < FORM_CC ? reg : 0), 0, code[s[first]].imm});
+        if (form >= FORM_CC) out.push_back(Instr{OP_ARG, 0, 0, 0, code[s[1]].imm});
+    }
+    code.resize(begin);
+    code.insert(code.end(), out.begin(), out.end());
+}
+
 inline bool ProgramBuilder::scope(const std::vector<Root> &roots) {
+    const size_t begin = code.size();
     // 1. reference counts inside the scope (number of parents + root uses)
     std::map<uint32_t, int> refs;
     std::vector<uint32_t> stack;
@@ -199,6 +276,7 @@ inline bool ProgramBuilder::scope(const std::vector<Root> &roots) {
         else code.push_back(Instr{OP_STORE, 0, (uint8_t)rr, 0, r.imm});
         release_use(r.node);
     }
+    fuse(begin);
     return true;
 }
 

@@ -486,18 +486,15 @@ static int32_t upload_table(DevPool &pool, const std::vector<T *> &host, T ***de
     ZKB_CUDA(cudaStreamSynchronize(st));
     return ZKB_OK;
 }
-// one program whose root i is STOREd to outs[i], uploaded with its output table and run over the 2^log_n rows of the d_cols table;
-// *nregs (if given) receives the program's register count
+// one program whose root i is STOREd to outs[i], uploaded with its output table and run over the 2^log_n rows of the d_cols table
 static int32_t run_store_program(zkb_ctx *ctx, uint32_t log_n, DevPool &pool, ExprBuilder &eb, const std::vector<uint32_t> &roots,
-                                 const std::vector<Fr *> &outs, const Fr *const *d_cols, const std::string &what, cudaStream_t st,
-                                 int *nregs = nullptr) {
+                                 const std::vector<Fr *> &outs, const Fr *const *d_cols, const std::string &what, cudaStream_t st) {
     ProgramBuilder pb(eb);
     std::vector<ProgramBuilder::Root> stores;
     for (size_t i = 0; i < roots.size(); ++i) stores.push_back({roots[i], ProgramBuilder::STORE, (uint32_t)i});
     if (!pb.scope(stores)) { set_error("%s: %s", what.c_str(), pb.error.c_str()); return ZKB_ERR_ARG; }
     DeviceProgram dp;
     ZKB_TRY(upload_program(pool, pb, eb, dp, st));
-    if (nregs) *nregs = dp.nregs;
     Fr **d_outs = nullptr;
     ZKB_TRY(upload_table(pool, outs, &d_outs, st));
     return expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, log_n, 1, 0, st);
@@ -1835,6 +1832,31 @@ extern "C" int32_t zkb_prove_finish(zkb_session *s, const uint64_t *z_blinds, co
 // ================================================================================================ C ABI: constraint interpreter
 // The gates of a CSF evaluated over caller columns by the prover's own compiler (translate, ProgramBuilder, quotient_gates) and
 // interpreter (expr_run_device): the hot kernel of a proof checked row by row against a reference evaluator.
+// The gate program of zkb_expr_eval_dev / zkb_expr_program (csf already validated and parsed into cs).  Mode 0: every gate a
+// STORE root of ONE CSE scope, like the lookup compression programs.  Mode 1: the gate part of evaluate_h's quotient program,
+// then one STOREACC with `scale`.
+static int32_t gate_program(const Csf &cs, int32_t mode, const uint64_t *challenges, const uint64_t y[4], const uint64_t scale[4],
+                            ExprBuilder &eb, ProgramBuilder &pb) {
+    ZKB_ARG(cs.nch == 0 || challenges);
+    std::vector<Fr> ch(cs.nch);
+    for (uint32_t i = 0; i < cs.nch; ++i) memcpy(ch[i].l, challenges + 4 * i, sizeof(Fr));
+    const SlotMap sm(cs);
+    std::vector<int64_t> memo(cs.nodes.size(), -1);
+    if (mode == 0) {
+        std::vector<ProgramBuilder::Root> roots;
+        for (size_t i = 0; i < cs.gates.size(); ++i) roots.push_back({translate(cs, cs.gates[i], eb, sm, ch, memo), ProgramBuilder::STORE, (uint32_t)i});
+        if (!pb.scope(roots)) { set_error("gates: %s", pb.error.c_str()); return ZKB_ERR_ARG; }
+        return ZKB_OK;
+    }
+    Fr yv, sv;
+    memcpy(yv.l, y, sizeof(Fr));
+    memcpy(sv.l, scale, sizeof(Fr));
+    const uint32_t y_idx = eb.const_slot(yv);
+    ZKB_TRY(quotient_gates(cs, ch, eb, pb, sm, memo, yv, y_idx));
+    pb.store_acc(0, eb.const_slot(sv));
+    return ZKB_OK;
+}
+
 extern "C" int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, int32_t mode, const uint64_t *challenges,
                                      const uint64_t y[4], const uint64_t scale[4], const uint64_t *const *columns_dev,
                                      uint64_t *const *outs_dev, uint32_t out_stride, uint32_t out_offset, uint32_t *nregs_out, void *stream) {
@@ -1844,45 +1866,40 @@ extern "C" int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t
     ZKB_TRY(zkb_csf_validate(csf, csf_words));
     Csf cs;
     parse_csf(csf, csf_words, cs);
-    ZKB_ARG(cs.nch == 0 || challenges);
-    std::vector<Fr> ch(cs.nch);
-    for (uint32_t i = 0; i < cs.nch; ++i) memcpy(ch[i].l, challenges + 4 * i, sizeof(Fr));
+    ExprBuilder eb;
+    ProgramBuilder pb(eb);
+    ZKB_TRY(gate_program(cs, mode, challenges, y, scale, eb, pb));
     cudaStream_t st = pick_stream(ctx, stream);
-    const SlotMap sm(cs);
     std::vector<Fr *> cols(cs.nf + cs.na + cs.ni);
     for (size_t i = 0; i < cols.size(); ++i) cols[i] = (Fr *)columns_dev[i];
+    std::vector<Fr *> outs(mode == 0 ? cs.gates.size() : 1);
+    for (size_t i = 0; i < outs.size(); ++i) outs[i] = (Fr *)outs_dev[i];
     DevPool pool;
     pool.ctx = ctx;
-    Fr **d_cols = nullptr;
+    Fr **d_cols = nullptr, **d_outs = nullptr;
+    DeviceProgram dp;
     ZKB_TRY(upload_table(pool, cols, &d_cols, st));
-    ExprBuilder eb;
-    std::vector<int64_t> memo(cs.nodes.size(), -1);
-    int nregs = 0;
-    if (mode == 0) {   // every gate one root of ONE CSE scope, like the lookup compression programs
-        std::vector<uint32_t> roots;
-        std::vector<Fr *> outs;
-        for (size_t i = 0; i < cs.gates.size(); ++i) {
-            roots.push_back(translate(cs, cs.gates[i], eb, sm, ch, memo));
-            outs.push_back((Fr *)outs_dev[i]);
-        }
-        ZKB_TRY(run_store_program(ctx, cs.k, pool, eb, roots, outs, d_cols, "gates", st, &nregs));
-    } else {           // the gate part of evaluate_h's quotient program, then one STOREACC with `scale`
-        Fr yv, sv;
-        memcpy(yv.l, y, sizeof(Fr));
-        memcpy(sv.l, scale, sizeof(Fr));
-        ProgramBuilder pb(eb);
-        const uint32_t y_idx = eb.const_slot(yv);
-        ZKB_TRY(quotient_gates(cs, ch, eb, pb, sm, memo, yv, y_idx));
-        pb.store_acc(0, eb.const_slot(sv));
-        DeviceProgram dp;
-        ZKB_TRY(upload_program(pool, pb, eb, dp, st));
-        nregs = dp.nregs;
-        Fr **d_outs = nullptr;
-        ZKB_TRY(upload_table(pool, std::vector<Fr *>{(Fr *)outs_dev[0]}, &d_outs, st));
-        ZKB_TRY(expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, cs.k, out_stride, out_offset, st));
-    }
+    ZKB_TRY(upload_table(pool, outs, &d_outs, st));
+    ZKB_TRY(upload_program(pool, pb, eb, dp, st));
+    ZKB_TRY(expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, cs.k, out_stride, out_offset, st));
     ZKB_CUDA(cudaStreamSynchronize(st));   // the program buffers go back to the context's block cache on return
-    if (nregs_out) *nregs_out = (uint32_t)nregs;
+    if (nregs_out) *nregs_out = (uint32_t)dp.nregs;
+    return ZKB_OK;
+}
+
+extern "C" int32_t zkb_expr_program(const uint32_t *csf, uint64_t csf_words, int32_t mode, const uint64_t *challenges, const uint64_t y[4],
+                                    const uint64_t scale[4], uint64_t *code_out, uint64_t cap, uint64_t *ncode_out, uint32_t *nregs_out) {
+    ZKB_ARG(csf && ncode_out && (mode == 0 || mode == 1) && (mode == 0 || (y && scale)) && (code_out || cap == 0));
+    ZKB_TRY(zkb_csf_validate(csf, csf_words));
+    Csf cs;
+    parse_csf(csf, csf_words, cs);
+    ExprBuilder eb;
+    ProgramBuilder pb(eb);
+    ZKB_TRY(gate_program(cs, mode, challenges, y, scale, eb, pb));
+    static_assert(sizeof(Instr) == sizeof(uint64_t), "one program word per instruction");
+    *ncode_out = pb.code.size();
+    if (nregs_out) *nregs_out = (uint32_t)pb.max_regs_used;
+    if (cap) memcpy(code_out, pb.code.data(), std::min<uint64_t>(cap, pb.code.size()) * sizeof(Instr));
     return ZKB_OK;
 }
 

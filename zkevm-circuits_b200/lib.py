@@ -76,6 +76,8 @@ SIGNATURES = {
     "zkb_csf_validate": (ctypes.c_int32, [_vp, ctypes.c_uint64]),
     "zkb_expr_eval_dev": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, ctypes.c_int32, _vp, _vp, _vp, _vp, _vp, ctypes.c_uint32,
                                            ctypes.c_uint32, ctypes.POINTER(ctypes.c_uint32), _vp]),
+    "zkb_expr_program": (ctypes.c_int32, [_vp, ctypes.c_uint64, ctypes.c_int32, _vp, _vp, _vp, _vp, ctypes.c_uint64,
+                                          ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint32)]),
     "zkb_check_witness_dev": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, _vp, _vp, _vp, _vp, ctypes.c_uint64, _vp, _vp, ctypes.c_uint32,
                                                ctypes.POINTER(ctypes.c_uint32), _vp]),
     "zkb_prove_begin": (ctypes.c_int32, [_vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),

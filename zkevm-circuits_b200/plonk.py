@@ -143,6 +143,24 @@ def expr_eval(cs, columns, mode=0, challenges=(), y=None, scale=None, out=None, 
     return outs, int(nregs.value)
 
 
+def expr_program(cs, mode=0, challenges=(), y=None, scale=None):
+    """Host only: the interpreter program expr_eval would run (zkb_expr_program), as (uint64 array, one word per instruction:
+    op | dst << 8 | a << 16 | b << 24 | imm << 32, register count)."""
+    from .lib import load_library
+    lib = load_library()
+    blob = cs.to_csf()
+    ch = np.ascontiguousarray(np.asarray(challenges, dtype=np.uint64).reshape(-1, 4))
+    yl = np.ascontiguousarray(np.asarray(y if y is not None else [0] * 4, dtype=np.uint64).reshape(4))
+    sl = np.ascontiguousarray(np.asarray(scale if scale is not None else [0] * 4, dtype=np.uint64).reshape(4))
+    args = [_vp(blob.ctypes.data), blob.size, int(mode), _vp(ch.ctypes.data) if ch.size else None,
+            _vp(yl.ctypes.data) if y is not None else None, _vp(sl.ctypes.data) if scale is not None else None]
+    ncode, nregs = ctypes.c_uint64(0), ctypes.c_uint32(0)
+    check(lib.zkb_expr_program(*args, None, 0, ctypes.byref(ncode), None))
+    code = np.zeros(ncode.value, dtype=np.uint64)
+    check(lib.zkb_expr_program(*args, _vp(code.ctypes.data), code.size, ctypes.byref(ncode), ctypes.byref(nregs)))
+    return code, int(nregs.value)
+
+
 R_MOD = 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001
 GATE, LOOKUP, COPY = 0, 1, 2
 Failure = namedtuple("Failure", "kind index sub row")   # zkb_check_record: sub = poisoned (gate) / input set (lookup) / 0 (copy)
