@@ -10,6 +10,7 @@
 // theta on the Lagrange domain (mv_lookup/prover.rs `prepare`).
 #pragma once
 #include <stdint.h>
+#include <algorithm>
 #include <array>
 #include <map>
 #include <string>
@@ -63,6 +64,9 @@ class ExprBuilder {
 public:
     std::vector<ENode> nodes;
     std::vector<Fr> consts;
+    // degree of each node as a polynomial in the columns, set as the node is interned (children come first): a column 1 (X, l_0,
+    // l_last and l_blind too, an upper bound), a constant 0, add / sub the larger operand's, mul the sum, neg its operand's
+    std::vector<uint32_t> degree;
 
     uint32_t col(uint32_t slot, int32_t rot) { return intern(0, slot, (uint32_t)rot); }
     uint32_t constant(const Fr &v) {
@@ -86,6 +90,22 @@ public:
         uint32_t n = constant(v);
         return nodes[n].a;
     }
+    // set used[slot] for every column slot read under `root`; `seen` (one entry per node) carries the visited nodes across calls
+    void columns(uint32_t root, std::vector<char> &seen, std::vector<char> &used) const {
+        std::vector<uint32_t> stack{root};
+        while (!stack.empty()) {
+            const uint32_t v = stack.back();
+            stack.pop_back();
+            if (seen[v]) continue;
+            seen[v] = 1;
+            const ENode &e = nodes[v];
+            if (e.kind == 0) used[e.a] = 1;
+            else if (e.kind >= 2) {
+                stack.push_back(e.a);
+                if (e.kind != 5) stack.push_back(e.b);
+            }
+        }
+    }
 
 private:
     std::map<std::tuple<uint8_t, uint32_t, uint32_t>, uint32_t> index;
@@ -95,6 +115,7 @@ private:
         auto it = index.find(key);
         if (it != index.end()) return it->second;
         nodes.push_back(ENode{kind, a, b});
+        degree.push_back(kind == 0 ? 1 : kind == 1 ? 0 : kind == 4 ? degree[a] + degree[b] : kind == 5 ? degree[a] : std::max(degree[a], degree[b]));
         index.emplace(key, (uint32_t)nodes.size() - 1);
         return (uint32_t)nodes.size() - 1;
     }

@@ -15,7 +15,8 @@
 // polynomials, coset evaluations, the quotient; only 64-byte commitments and 32-byte evaluations return to the host.
 //
 // Design points (not upstream's): the quotient is evaluated coset-part by coset-part (extended domain = E cosets of
-// size n, SURVEY 8e) by ONE fused interpreter kernel per part; all scans / inversions / evaluations are parallel kernels.
+// size n, SURVEY 8e) by one fused interpreter launch per degree group on the part, each group only on the parts its degree
+// needs (QuotientGroups); all scans / inversions / evaluations are parallel kernels.
 #include "common.cuh"
 #include "expr.cuh"
 #include "blake2b.h"
@@ -117,12 +118,13 @@ __global__ void sub_low_kernel(Fr *__restrict__ out, const Fr *__restrict__ low,
     if (i < k) fp_store(out + i, fp_sub(fp_load(out + i), fp_load(low + i)));
 }
 
-// out[j + E * i] = parts[j * n + i]  (coset parts gathered as rows -> extended-domain order)
-__global__ void interleave_parts_kernel(const Fr *__restrict__ parts, Fr *__restrict__ out, uint32_t log_n, uint32_t E) {
+// out[j + m * i] = slab[rows[j] * n + i]  (a quotient group's coset parts gathered as rows -> its order on zeta D_{mn})
+__global__ void interleave_rows_kernel(const Fr *__restrict__ slab, const uint32_t *__restrict__ rows, Fr *__restrict__ out, uint32_t log_n,
+                                       uint32_t m) {
     const uint64_t idx = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
-    if (idx >= ((uint64_t)E << log_n)) return;
-    const uint64_t j = idx % E, i = idx / E;
-    fp_store(out + idx, fp_load(parts + (j << log_n) + i));
+    if (idx >= ((uint64_t)m << log_n)) return;
+    const uint64_t j = idx % m, i = idx / m;
+    fp_store(out + idx, fp_load(slab + ((uint64_t)rows[j] << log_n) + i));
 }
 
 // ---- multiplicities of the mv-lookup: open-addressing hash table keyed by the 32-byte compressed table value --------
@@ -1084,6 +1086,7 @@ struct ProofState {
     Fr *random_poly = nullptr;
     std::vector<Fr *> adv_polys, z_polys, phi_polys, m_polys;
     Fr *h_ext = nullptr;                     // h on the extended domain; after the inverse transform, qdeg pieces of n coefficients
+    std::vector<Fr *> h_group;               // quotient group g's values on zeta D_{mn}, m = 2^g (the top one is h_ext; null: empty)
     std::vector<Fr *> h_pieces;
     std::map<int64_t, Fr> point_of;          // rotation -> x * omega^rot
     std::map<std::pair<int, int64_t>, Fr> eval_of;
@@ -1332,12 +1335,84 @@ static int32_t coefficient_forms(zkb_session *s, ProofState &ps) {
     return to_coeff_dealt(s, ps.lk_m, ps.m_polys);
 }
 
+// The quotient numerator split by degree.  Constraint i of T contributes c_i y^(T-1-i).  A constraint of degree d vanishes on H,
+// so c_i / Z_H has degree at most d (n - 1) - n < (d - 1) n: its share of h is fixed by its values on the m n points zeta D_{mn},
+// m the smallest power of two >= max(d - 1, 1), at most E.  Those points are the coset parts j = 0 mod E/m (part (E/m) j' has the
+// generator zeta w_{mn}^j').  Group g collects the constraints with m = 2^g into a program of its own, keeping the global y order:
+// its Horner steps are y^(i - i_prev) (i_prev the group's previous constraint), and the tail y^(T-1-i_last) goes into the STOREACC
+// scale.  The groups' h_g add up to h coefficient for coefficient, so the proof does not change.  Putting a constraint in a larger
+// group is always correct: a folded selector run takes its highest-degree member's group.  With one group (E = 1) every gap is 1
+// and the single program of before comes out unchanged.
+struct QuotientGroups {
+    ExprBuilder &eb;
+    const Fr y;
+    const uint32_t E;
+    const std::vector<ProgramBuilder *> pb;     // group g (m = 2^g) writes pb[g]; log2(E) + 1 of them
+    std::vector<int64_t> last;                  // global index of the group's latest constraint, -1 before its first
+    std::vector<uint32_t> count;                // constraints per group
+    std::vector<std::vector<uint32_t>> reads;   // per group, nodes whose columns it reads (they decide the coset NTTs)
+    int64_t next = 0;                           // global index of the next constraint
+    std::string error;
+
+    QuotientGroups(ExprBuilder &eb, const Fr &y, uint32_t E, std::vector<ProgramBuilder *> pb)
+        : eb(eb), y(y), E(E), pb(std::move(pb)), last(this->pb.size(), -1), count(this->pb.size(), 0), reads(this->pb.size()) {
+        eb.const_slot(y);   // y is the first constant, as the Horner steps are almost all y^1
+    }
+    uint32_t group_of(uint32_t degree) const {
+        const uint32_t need = std::max<uint32_t>(degree, 2) - 1;
+        uint32_t g = 0;
+        while ((1u << g) < need && (1u << g) < E) ++g;
+        return g;
+    }
+    // y^(gap) for a group's next constraint at global index i; a group's first step multiplies a zero accumulator
+    uint32_t step(uint32_t g, int64_t i) { return eb.const_slot(fp_pow_u64(y, last[g] < 0 ? 1 : (uint64_t)(i - last[g]))); }
+    bool emit(uint32_t g, const std::vector<ProgramBuilder::Root> &r) {
+        if (pb[g]->scope(r)) return true;
+        error = pb[g]->error;
+        return false;
+    }
+    // constraints in order, sharing one CSE scope per group (a lookup's three roots: the l_0 / l_last ones have degree 2)
+    bool scope(const std::vector<uint32_t> &nodes) {
+        std::vector<std::vector<ProgramBuilder::Root>> per(pb.size());
+        for (uint32_t v : nodes) {
+            const uint32_t g = group_of(eb.degree[v]);
+            per[g].push_back({v, ProgramBuilder::HORNER, step(g, next)});
+            reads[g].push_back(v);
+            last[g] = next++;
+            count[g]++;
+        }
+        for (uint32_t g = 0; g < pb.size(); ++g)
+            if (!per[g].empty() && !emit(g, per[g])) return false;
+        return true;
+    }
+    // a folded selector run sel * rests[t]: acc2 Horner-steps by y inside the run, FOLD steps acc by y^(s - i_prev - 1 + r)
+    bool run(const std::vector<uint32_t> &rests, uint32_t sel) {
+        uint32_t d = 0;
+        for (uint32_t v : rests) d = std::max(d, eb.degree[v]);
+        const uint32_t g = group_of(eb.degree[sel] + d);
+        const int64_t s = next, r = (int64_t)rests.size();
+        for (uint32_t v : rests)
+            if (!emit(g, {{v, ProgramBuilder::HORNER2, eb.const_slot(y)}})) return false;
+        const uint32_t fold = eb.const_slot(fp_pow_u64(y, (uint64_t)(last[g] < 0 ? r : s - last[g] - 1 + r)));
+        if (!emit(g, {{sel, ProgramBuilder::FOLD, fold}})) return false;
+        reads[g].push_back(sel);
+        reads[g].insert(reads[g].end(), rests.begin(), rests.end());
+        last[g] = s + r - 1;
+        next += r;
+        count[g] += (uint32_t)r;
+        return true;
+    }
+    // y^(T-1-i_last) of a non-empty group, once every constraint is in
+    Fr tail(uint32_t g) const { return fp_pow_u64(y, (uint64_t)(next - 1 - last[g])); }
+};
+
 // Gate polynomials of the quotient program, Horner in y in constraint-system order.  Circuits multiply whole groups of constraints
 // by one selector (`q_enable * constraint`), so runs of CONSECUTIVE gates of the form fixed(col, rot) * t_j are folded exactly:
 //   (..(acc y + f t_1) y + ..) y + f t_r  =  acc y^r + f (t_1 y^(r-1) + .. + t_r)
 // -- the same field element (distributivity is exact mod r), one multiply per gate less than the term-by-term form.
-static int32_t quotient_gates(const Csf &cs, const std::vector<Fr> &challenges, ExprBuilder &qeb, ProgramBuilder &qpb, const SlotMap &sm,
-                              std::vector<int64_t> &memo, const Fr &y, uint32_t y_idx) {
+static int32_t quotient_gates(const Csf &cs, const std::vector<Fr> &challenges, QuotientGroups &qg, const SlotMap &sm,
+                              std::vector<int64_t> &memo) {
+    ExprBuilder &qeb = qg.eb;
     auto selector_split = [&](uint32_t gnode, uint32_t &sel, uint32_t &rest) -> bool {
         const auto &nd = cs.nodes[gnode];
         if (nd[0] != N_MUL) return false;
@@ -1356,24 +1431,26 @@ static int32_t quotient_gates(const Csf &cs, const std::vector<Fr> &challenges, 
             while (gi + run < cs.gates.size() && run < 4096 && selector_split(cs.gates[gi + run], s2, r2) && same_query(sel, s2)) ++run;
         }
         if (run < 2) {
-            if (!qpb.scope({{translate(cs, cs.gates[gi], qeb, sm, challenges, memo), ProgramBuilder::HORNER, y_idx}})) { set_error("gate: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
+            if (!qg.scope({translate(cs, cs.gates[gi], qeb, sm, challenges, memo)})) { set_error("gate: %s", qg.error.c_str()); return ZKB_ERR_ARG; }
             ++gi;
             continue;
         }
+        // the whole run is translated first: its degree picks the group (the selector is a column: it adds no constant)
+        std::vector<uint32_t> rests(run);
         for (size_t t = 0; t < run; ++t) {
             uint32_t s2 = 0, r2 = 0;
             selector_split(cs.gates[gi + t], s2, r2);
-            if (!qpb.scope({{translate(cs, r2, qeb, sm, challenges, memo), ProgramBuilder::HORNER2, y_idx}})) { set_error("gate: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
+            rests[t] = translate(cs, r2, qeb, sm, challenges, memo);
         }
-        const uint32_t yr_idx = qeb.const_slot(fp_pow_u64(y, run));
-        if (!qpb.scope({{translate(cs, sel, qeb, sm, challenges, memo), ProgramBuilder::FOLD, yr_idx}})) { set_error("gate: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
+        if (!qg.run(rests, translate(cs, sel, qeb, sm, challenges, memo))) { set_error("gate: %s", qg.error.c_str()); return ZKB_ERR_ARG; }
         gi += run;
     }
     return ZKB_OK;
 }
 
-// evaluation.rs evaluate_h: the quotient numerator program (gates, permutation, lookups, in upstream's y-Horner order), then
-// per coset part j the coset NTTs of every polynomial not in the pk's coset cache and ONE interpreter launch, x 1/((zeta w^j)^n - 1)
+// evaluation.rs evaluate_h: the quotient numerator (gates, permutation, lookups, in upstream's y-Horner order) as one program per
+// degree group (QuotientGroups), then per coset part j the coset NTTs of the polynomials its groups read that the pk's coset cache
+// does not hold, and one interpreter launch per group on the part, x y^(T-1-i_last) / ((zeta w^j)^n - 1)
 static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
     zkb_pk *pk = s->pk;
     zkb_ctx *ctx = pk->ctx;
@@ -1404,19 +1481,24 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
     const uint32_t q_llast = q_l0 + 1, q_lblind = q_l0 + 2, q_x = q_l0 + 3;
     ZKB_ARG(qpolys.size() < 65536);
 
+    const uint32_t E = pk->E;
+    uint32_t G = 1;   // groups m = 1, 2, .., E
+    while ((1u << (G - 1)) < E) ++G;
     ExprBuilder qeb;
-    ProgramBuilder qpb(qeb);
-    const uint32_t y_idx = qeb.const_slot(ps.y);
+    std::vector<ProgramBuilder> qpbs(G, ProgramBuilder(qeb));
+    std::vector<ProgramBuilder *> qpb_ptrs;
+    for (auto &p : qpbs) qpb_ptrs.push_back(&p);
+    QuotientGroups qg(qeb, ps.y, E, qpb_ptrs);
     std::vector<int64_t> memo(cs.nodes.size(), -1);
-    ZKB_TRY(quotient_gates(cs, s->challenges, qeb, qpb, sm, memo, ps.y, y_idx));
+    ZKB_TRY(quotient_gates(cs, s->challenges, qg, sm, memo));
     auto lactive = [&]() { return qeb.sub(qeb.sub(qeb.constant(one), qeb.col(q_llast, 0)), qeb.col(q_lblind, 0)); };
     if (pk->nsets) {
         const uint32_t z0 = qeb.col(q_z0, 0), zl = qeb.col(q_z0 + pk->nsets - 1, 0);
-        if (!qpb.scope({{qeb.mul(qeb.sub(qeb.constant(one), z0), qeb.col(q_l0, 0)), ProgramBuilder::HORNER, y_idx}})) return ZKB_ERR_ARG;
-        if (!qpb.scope({{qeb.mul(qeb.sub(qeb.mul(zl, zl), zl), qeb.col(q_llast, 0)), ProgramBuilder::HORNER, y_idx}})) return ZKB_ERR_ARG;
+        if (!qg.scope({qeb.mul(qeb.sub(qeb.constant(one), z0), qeb.col(q_l0, 0))})) return ZKB_ERR_ARG;
+        if (!qg.scope({qeb.mul(qeb.sub(qeb.mul(zl, zl), zl), qeb.col(q_llast, 0))})) return ZKB_ERR_ARG;
         for (uint32_t i = 1; i < pk->nsets; ++i) {
             const uint32_t t = qeb.mul(qeb.sub(qeb.col(q_z0 + i, 0), qeb.col(q_z0 + i - 1, -(int32_t)(cs.bf + 1))), qeb.col(q_l0, 0));
-            if (!qpb.scope({{t, ProgramBuilder::HORNER, y_idx}})) return ZKB_ERR_ARG;
+            if (!qg.scope({t})) return ZKB_ERR_ARG;
         }
         const Fr delta = perm_delta();
         Fr delta_pow = one;
@@ -1428,7 +1510,7 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
                 right = qeb.mul(right, qeb.add(qeb.add(v, qeb.mul(qeb.col(q_x, 0), qeb.constant(fp_mul(ps.beta, delta_pow)))), qeb.constant(ps.gamma)));
                 delta_pow = fp_mul(delta_pow, delta);
             }
-            if (!qpb.scope({{qeb.mul(qeb.sub(left, right), lactive()), ProgramBuilder::HORNER, y_idx}})) { set_error("permutation: %s", qpb.error.c_str()); return ZKB_ERR_ARG; }
+            if (!qg.scope({qeb.mul(qeb.sub(left, right), lactive())})) { set_error("permutation: %s", qg.error.c_str()); return ZKB_ERR_ARG; }
         }
     }
     for (size_t l = 0; l < cs.lookups.size(); ++l) {
@@ -1455,28 +1537,31 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
         const uint32_t phi = qeb.col(q_phi0 + (uint32_t)l, 0), phi_next = qeb.col(q_phi0 + (uint32_t)l, 1), m = qeb.col(q_m0 + (uint32_t)l, 0);
         const uint32_t lhs = qeb.mul(qeb.mul(tb, prod), qeb.sub(phi_next, phi));
         const uint32_t rhs = qeb.sub(qeb.mul(tb, ssum), qeb.mul(m, prod));
-        std::vector<ProgramBuilder::Root> roots = {{qeb.mul(phi, qeb.col(q_l0, 0)), ProgramBuilder::HORNER, y_idx},
-                                                   {qeb.mul(phi, qeb.col(q_llast, 0)), ProgramBuilder::HORNER, y_idx},
-                                                   {qeb.mul(qeb.sub(lhs, rhs), lactive()), ProgramBuilder::HORNER, y_idx}};
-        if (!qpb.scope(roots)) { set_error("lookup %zu: %s", l, qpb.error.c_str()); return ZKB_ERR_ARG; }
+        if (!qg.scope({qeb.mul(phi, qeb.col(q_l0, 0)), qeb.mul(phi, qeb.col(q_llast, 0)), qeb.mul(qeb.sub(lhs, rhs), lactive())})) {
+            set_error("lookup %zu: %s", l, qg.error.c_str());
+            return ZKB_ERR_ARG;
+        }
     }
-    // one STOREACC per coset part (the scale constant differs): the device code buffer holds the common body + one trailing
-    // STOREACC slot that is rewritten per part
-    std::vector<uint32_t> tinv_idx(pk->E);
-    for (uint32_t j = 0; j < pk->E; ++j) tinv_idx[j] = qeb.const_slot(pk->t_inv[j]);
-    const size_t base_len = qpb.code.size();
-    DeviceProgram qdp;
-    qpb.store_acc(0, tinv_idx[0]);
-    ZKB_TRY(upload_program(pool, qpb, qeb, qdp, st));
-    trace.mark("quotient program build+upload");
-
-    // evaluate h on the extended domain, part by part
-    Fr *slab, *pows;
-    ZKB_TRY(pool.fr(qpolys.size() * n, &slab));
-    ZKB_TRY(pool.fr(n, &pows));
-    ZKB_TRY(pool.fr(pk->N, &ps.h_ext));
-    std::vector<Fr *> qcols(qpolys.size());
-    for (size_t i = 0; i < qpolys.size(); ++i) qcols[i] = slab + i * n;
+    // group g runs on the coset parts j = 0 mod E/m, m = 2^g: every group on part 0, only the top one (m = E) on the odd parts
+    auto on_part = [&](uint32_t g, uint32_t j) { return j % (E >> g) == 0; };
+    std::vector<uint32_t> groups;   // the non-empty ones
+    for (uint32_t g = 0; g < G; ++g)
+        if (qg.count[g]) groups.push_back(g);
+    // one program per group.  Its device code buffer holds the body + one trailing STOREACC slot, rewritten per part with the scale
+    // t_inv[j] y^(T-1-i_last)
+    std::vector<std::vector<uint32_t>> scale_idx(G, std::vector<uint32_t>(E, 0));
+    for (uint32_t g : groups) {
+        const Fr tail = qg.tail(g);
+        for (uint32_t j = 0; j < E; ++j)
+            if (on_part(g, j)) scale_idx[g][j] = qeb.const_slot(fp_mul(pk->t_inv[j], tail));
+    }
+    std::vector<DeviceProgram> qdp(G);
+    std::vector<size_t> base_len(G, 0);
+    for (uint32_t g : groups) {
+        base_len[g] = qpbs[g].code.size();
+        qpbs[g].store_acc(0, scale_idx[g][0]);
+        ZKB_TRY(upload_program(pool, qpbs[g], qeb, qdp[g], st));
+    }
     // slots served from the pk's coset cache: fixed, sigma, l0 / l_last / l_blind / X
     const bool cached = !pk->coset_cache.empty();
     std::vector<int> cache_idx(qpolys.size(), -1);
@@ -1486,53 +1571,123 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
         for (size_t i = 0; i < cs.perm.size(); ++i) cache_idx[sm.sigma0 + i] = ci++;
         cache_idx[q_l0] = ci++; cache_idx[q_llast] = ci++; cache_idx[q_lblind] = ci++; cache_idx[q_x] = ci++;
     }
-    std::vector<Fr *> ntt_src, ntt_dst;
-    for (size_t i = 0; i < qpolys.size(); ++i) {
-        if (cache_idx[i] < 0) { ntt_src.push_back(qpolys[i]); ntt_dst.push_back(qcols[i]); }
+    // the largest group reading each slot: a polynomial outside the cache is transformed on that group's parts (a smaller group's
+    // parts are a subset of them), and not at all when no constraint reads it
+    std::vector<int> reader(qpolys.size(), -1);
+    {
+        std::vector<char> seen(qeb.nodes.size());
+        for (uint32_t g : groups) {
+            std::fill(seen.begin(), seen.end(), 0);
+            std::vector<char> used(qpolys.size(), 0);
+            for (uint32_t v : qg.reads[g]) qeb.columns(v, seen, used);
+            for (size_t i = 0; i < used.size(); ++i)
+                if (used[i]) reader[i] = (int)g;
+        }
     }
-    Fr **d_qcols = nullptr, **d_hout = nullptr;
-    ZKB_TRY(pool.alloc(qcols.size() * sizeof(Fr *) + 8, (void **)&d_qcols));
-    std::vector<Fr *> hout{ps.h_ext};
-    ZKB_TRY(upload_table(pool, hout, &d_hout, st));
-    // multi-GPU: coset parts are dealt in contiguous blocks; a rank writes its parts as contiguous n-element rows of h_parts, the rows
-    // are all-gathered and interleaved into the extended-domain order h_ext[j + E i] the inverse transform expects
-    const Deal dq(ctx, pk->E);
-    Fr *h_parts = nullptr;
+    if (trace.on) {
+        for (uint32_t g : groups) {
+            size_t instrs = 0, ntts = 0;
+            for (const Instr &in : qpbs[g].code) instrs += in.op != OP_ARG;
+            for (size_t i = 0; i < qpolys.size(); ++i) ntts += cache_idx[i] < 0 && reader[i] == (int)g;
+            fprintf(stderr, "[zkb trace] quotient group m = %-2u %6u constraints %7zu instructions/row %5zu coset NTTs\n", 1u << g, qg.count[g],
+                    instrs, ntts << g);
+        }
+    }
+    trace.mark("quotient program build+upload");
+
+    // evaluate h part by part: group g's value at zeta w_{mn}^(j' + m i) is h_g[j' + m i], part j = (E/m) j'; the top group's h_g is h_ext
+    Fr *slab, *pows;
+    ZKB_TRY(pool.fr(qpolys.size() * n, &slab));
+    ZKB_TRY(pool.fr(n, &pows));
+    ZKB_TRY(pool.fr(pk->N, &ps.h_ext));
+    ps.h_group.assign(G, nullptr);
+    for (uint32_t g : groups) {
+        if (g + 1 == G) ps.h_group[g] = ps.h_ext;
+        else ZKB_TRY(pool.fr(n << g, &ps.h_group[g]));
+    }
+    std::vector<Fr *> qcols(qpolys.size());
+    for (size_t i = 0; i < qpolys.size(); ++i) qcols[i] = slab + i * n;
+    // multi-GPU: coset parts are dealt in contiguous blocks.  A rank writes one n-element row of rows_slab per (part, group on it),
+    // parts in order from row rank * blk_rows, so one all-gather of blk_rows rows per rank completes the slab; each group's rows are
+    // then interleaved into its order h_g[j' + m i]
+    const Deal dq(ctx, E);
+    std::vector<std::vector<uint32_t>> row_of(G, std::vector<uint32_t>(E, 0));
+    size_t blk_rows = 0;
+    Fr *rows_slab = nullptr;
     if (dq.on) {
-        ZKB_TRY(pool.fr(dq.padded() * n, &h_parts));
-        std::vector<Fr *> hp{h_parts};
-        ZKB_CUDA(cudaMemcpyAsync(d_hout, hp.data(), sizeof(Fr *), cudaMemcpyHostToDevice, st));
-        ZKB_CUDA(cudaStreamSynchronize(st));
+        std::vector<size_t> next_row(dq.P, 0);   // rows per rank, then the next free row of each rank
+        for (uint32_t j = 0; j < E; ++j)
+            for (uint32_t g : groups) next_row[j / dq.blk] += on_part(g, j);
+        blk_rows = *std::max_element(next_row.begin(), next_row.end());
+        for (int r = 0; r < dq.P; ++r) next_row[r] = (size_t)r * blk_rows;
+        for (uint32_t j = 0; j < E; ++j)
+            for (uint32_t g : groups)
+                if (on_part(g, j)) row_of[g][j] = (uint32_t)next_row[j / dq.blk]++;
+        ZKB_TRY(pool.fr((size_t)dq.P * blk_rows * n, &rows_slab));
     }
-    for (uint32_t j = 0; j < pk->E; ++j) {
+    std::vector<Fr **> d_hout(G, nullptr);
+    for (uint32_t g : groups) ZKB_TRY(upload_table(pool, std::vector<Fr *>{dq.on ? rows_slab : ps.h_group[g]}, &d_hout[g], st));
+    Fr **d_qcols = nullptr;
+    ZKB_TRY(pool.alloc(qcols.size() * sizeof(Fr *) + 8, (void **)&d_qcols));
+    for (uint32_t j = 0; j < E; ++j) {
         if (!dq.mine(j)) continue;
-        ZKB_TRY(fr_powers_device(ctx, pk->coset_gen(j), n, pows, st));
-        ZKB_TRY(ntt_many(pk, ntt_src, ntt_dst, pk->omega, nullptr, pows, st));
+        std::vector<Fr *> ntt_src, ntt_dst;
+        for (size_t i = 0; i < qpolys.size(); ++i)
+            if (cache_idx[i] < 0 && reader[i] >= 0 && on_part((uint32_t)reader[i], j)) { ntt_src.push_back(qpolys[i]); ntt_dst.push_back(qcols[i]); }
+        if (!ntt_src.empty()) {
+            ZKB_TRY(fr_powers_device(ctx, pk->coset_gen(j), n, pows, st));
+            ZKB_TRY(ntt_many(pk, ntt_src, ntt_dst, pk->omega, nullptr, pows, st));
+        }
         std::vector<Fr *> cols_j = qcols;
         if (cached)
             for (size_t i = 0; i < qpolys.size(); ++i)
                 if (cache_idx[i] >= 0) cols_j[i] = pk->coset_cache[j][cache_idx[i]];
-        Instr tail{OP_STOREACC, 0, 0, 0, 0u | (tinv_idx[j] << 8)};
         ZKB_CUDA(cudaMemcpyAsync(d_qcols, cols_j.data(), cols_j.size() * sizeof(Fr *), cudaMemcpyHostToDevice, st));
-        ZKB_CUDA(cudaMemcpyAsync(qdp.code + base_len, &tail, sizeof(Instr), cudaMemcpyHostToDevice, st));
-        if (dq.on) ZKB_TRY(expr_run_device(ctx, qdp.code, qdp.ncode, qdp.nregs, d_qcols, qdp.consts, d_hout, k, 1, (uint32_t)((uint64_t)j * n), st));
-        else ZKB_TRY(expr_run_device(ctx, qdp.code, qdp.ncode, qdp.nregs, d_qcols, qdp.consts, d_hout, k, pk->E, j, st));
-        ZKB_CUDA(cudaStreamSynchronize(st));  // `tail` and `cols_j` live on the stack
+        std::vector<Instr> tails(G);
+        for (uint32_t g : groups) {
+            if (!on_part(g, j)) continue;
+            tails[g] = Instr{OP_STOREACC, 0, 0, 0, 0u | (scale_idx[g][j] << 8)};
+            ZKB_CUDA(cudaMemcpyAsync(qdp[g].code + base_len[g], &tails[g], sizeof(Instr), cudaMemcpyHostToDevice, st));
+            const DeviceProgram &dp = qdp[g];
+            if (dq.on) ZKB_TRY(expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_qcols, dp.consts, d_hout[g], k, 1, (uint32_t)(row_of[g][j] * n), st));
+            else ZKB_TRY(expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_qcols, dp.consts, d_hout[g], k, 1u << g, j / (E >> g), st));
+        }
+        ZKB_CUDA(cudaStreamSynchronize(st));  // `tails` and `cols_j` live on the stack
     }
     if (dq.on) {
-        ZKB_TRY(deal_gather(ctx, dq, h_parts, n * sizeof(Fr), st));
-        interleave_parts_kernel<<<(unsigned)((pk->N + 255) / 256), 256, 0, st>>>(h_parts, ps.h_ext, k, pk->E);
-        ctx->launches++;
+        ZKB_TRY(comm_allgather(ctx, rows_slab + (size_t)dq.rank * blk_rows * n, rows_slab, blk_rows * n * sizeof(Fr), st));
+        std::vector<std::vector<uint32_t>> rows(G);
+        for (uint32_t g : groups) {
+            for (uint32_t jj = 0; jj < (1u << g); ++jj) rows[g].push_back(row_of[g][jj * (E >> g)]);
+            uint32_t *d_rows = nullptr;
+            ZKB_TRY(pool.alloc(rows[g].size() * sizeof(uint32_t), (void **)&d_rows));
+            ZKB_CUDA(cudaMemcpyAsync(d_rows, rows[g].data(), rows[g].size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st));
+            interleave_rows_kernel<<<(unsigned)(((n << g) + 255) / 256), 256, 0, st>>>(rows_slab, d_rows, ps.h_group[g], k, 1u << g);
+            ctx->launches++;
+        }
+        ZKB_CUDA(cudaStreamSynchronize(st));  // `rows` lives on the stack
     }
     return ZKB_OK;
 }
 
 // vanishing/prover.rs construct: extended_to_coeff (inverse NTT over the extended domain with 1/N and the zeta coset undone), the
-// qdeg pieces of n coefficients committed against g, then x
+// qdeg pieces of n coefficients committed against g, then x.  Each smaller quotient group's h_g comes back from zeta D_{mn} with an
+// inverse NTT of size m n (1/(mn), zeta undone) and is added into the first m n coefficients.
 static int32_t vanishing_construct(zkb_session *s, ProofState &ps) {
     zkb_pk *pk = s->pk;
     cudaStream_t st = pk->ctx->stream;
-    ZKB_TRY(ntt_fr_device(pk->ctx, ps.h_ext, ps.h_ext, pk->ext_k, pk->ext_omega_inv, &pk->N_inv, 2, nullptr, st));
+    const uint32_t G = (uint32_t)ps.h_group.size();
+    if (ps.h_group[G - 1]) ZKB_TRY(ntt_fr_device(pk->ctx, ps.h_ext, ps.h_ext, pk->ext_k, pk->ext_omega_inv, &pk->N_inv, 2, nullptr, st));
+    else ZKB_CUDA(cudaMemsetAsync(ps.h_ext, 0, pk->N * sizeof(Fr), st));
+    std::vector<Fr> mn_inv(G);
+    for (uint32_t g = 0; g + 1 < G; ++g) {
+        if (!ps.h_group[g]) continue;
+        const uint64_t mn = pk->n << g;
+        mn_inv[g] = fp_inv(fr_from_u64(mn));
+        ZKB_TRY(ntt_fr_device(pk->ctx, ps.h_group[g], ps.h_group[g], pk->k + g, fp_pow_u64(pk->ext_omega_inv, pk->E >> g), &mn_inv[g], 2, nullptr, st));
+        ZKB_TRY(zkb_field_binop_dev(pk->ctx, 0, 0, (const uint64_t *)ps.h_ext, (const uint64_t *)ps.h_group[g], (uint64_t *)ps.h_ext, mn, st));
+    }
+    ZKB_CUDA(cudaStreamSynchronize(st));   // `mn_inv` lives on the stack
     for (uint32_t i = 0; i < pk->qdeg; ++i) ps.h_pieces.push_back(ps.h_ext + (size_t)i * pk->n);
     ZKB_TRY(commit_write(s, ps.h_pieces, BASIS_G, st));
     ps.x = tr_squeeze(s);
@@ -1851,8 +2006,8 @@ static int32_t gate_program(const Csf &cs, int32_t mode, const uint64_t *challen
     Fr yv, sv;
     memcpy(yv.l, y, sizeof(Fr));
     memcpy(sv.l, scale, sizeof(Fr));
-    const uint32_t y_idx = eb.const_slot(yv);
-    ZKB_TRY(quotient_gates(cs, ch, eb, pb, sm, memo, yv, y_idx));
+    QuotientGroups qg(eb, yv, 1, {&pb});   // one group: every Horner gap is 1
+    ZKB_TRY(quotient_gates(cs, ch, qg, sm, memo));
     pb.store_acc(0, eb.const_slot(sv));
     return ZKB_OK;
 }
