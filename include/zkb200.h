@@ -132,6 +132,46 @@ ZKB_API int32_t zkb_srs_commit_host(zkb_srs *srs, int32_t basis, const uint64_t 
 ZKB_API int32_t zkb_srs_commit_batch_dev(zkb_srs *srs, int32_t basis, const uint64_t *const *scalar_cols_dev, uint32_t batch, uint64_t n,
                                          uint64_t *out_affine, void *stream);
 
+/* ---- params file points: ParamsKZG::read_custom / write_custom (halo2_proofs src/poly/kzg/commitment.rs) --------------------------
+ * A params file is 4 B k (u32 LE) | g: 2^k G1 | g_lagrange: 2^k G1 | g2 | s_g2, each point in the SerdeFormat the caller names (the
+ * reference loader prover/src/utils.rs load_params checks the length 4 + 2 * 2^k * g1 + 2 * g2 bytes):
+ *   format 0 Processed          G1 32 B: LE canonical x, bit 6 of byte 31 = canonical y & 1, bit 7 = 0, identity = 32 zero bytes (the
+ *                               G1Affine::to_bytes of zkb_msm_g1_*: pinned by the reference fixture's vk and proof points).
+ *                               G2 64 B: x.c0 || x.c1, LE canonical; bit 6 of byte 63 = parity of canonical y.c0 (of y.c1 when
+ *                               y.c0 = 0), bit 7 = 0, identity = 64 zero bytes.  This G2 convention follows upstream halo2curves
+ *                               and is NOT pinned by any fixture here; zkb_g2_decode_host and zkb_g2_encode_host share it.
+ *   format 1 RawBytes           G1 64 B / G2 128 B: the in-memory point (Montgomery limbs; G2 x.c0, x.c1, y.c0, y.c1); decoding checks
+ *                               every limb set < q and the curve equation ((0, 0) is the identity).
+ *   format 2 RawBytesUnchecked  the same bytes, copied without a check.
+ * zkb_g1_decode  n encoded points -> n G1Affine.  in and out_affine may each be host or device pointers (device pointers 16-byte
+ *                aligned); host buffers are streamed in chunks of ZKB_SERDE_CHUNK_POINTS through pinned double buffers, so the whole
+ *                input and output never need to be on the device.  A bad point is written as (0, 0); *rep receives the first bad
+ *                index (UINT64_MAX when none), the exact number of bad points and the reason of the first one, the same on every
+ *                run.  Returns ZKB_OK whether or not points are bad (bad points are data), ZKB_ERR_ARG for a bad format or pointer.
+ *                Work queued on `stream` before the call is complete before it reads `in`; synchronises `stream`.
+ * zkb_g1_encode  n G1Affine -> n encoded points (Processed: 32 B, raw formats: 64 B); same pointer rules; synchronises `stream`.
+ * zkb_g2_decode_host / zkb_g2_encode_host   one G2 point (g2, s_g2 of a file), host memory only, no device needed; *status receives the
+ *                reason code (0 = good; a bad point is written as zeros).                                                          */
+#define ZKB_SERDE_PROCESSED 0
+#define ZKB_SERDE_RAW_BYTES 1
+#define ZKB_SERDE_RAW_BYTES_UNCHECKED 2
+#define ZKB_SERDE_OK 0
+#define ZKB_SERDE_BAD_FLAGS 1        /* bit 7 of the last byte set */
+#define ZKB_SERDE_NON_CANONICAL 2    /* a coordinate (Processed: x; raw: any limb set) >= q */
+#define ZKB_SERDE_NOT_ON_CURVE 3     /* Processed: x^3 + b has no square root; raw: y^2 != x^3 + b */
+#define ZKB_SERDE_CHUNK_POINTS (1u << 20)
+typedef struct zkb_decode_report {
+    uint64_t first_bad;   /* index of the first bad point, UINT64_MAX when every point is good */
+    uint64_t count;       /* number of bad points */
+    uint32_t reason;      /* ZKB_SERDE_* reason of the first bad point */
+    uint32_t reserved;
+} zkb_decode_report;
+ZKB_API int32_t zkb_g1_decode(zkb_ctx *ctx, int32_t format, const uint8_t *in, uint64_t n, uint64_t *out_affine, zkb_decode_report *rep,
+                              void *stream);
+ZKB_API int32_t zkb_g1_encode(zkb_ctx *ctx, int32_t format, const uint64_t *in_affine, uint64_t n, uint8_t *out, void *stream);
+ZKB_API int32_t zkb_g2_decode_host(int32_t format, const uint8_t *in, uint64_t out[16], int32_t *status);
+ZKB_API int32_t zkb_g2_encode_host(int32_t format, const uint64_t in[16], uint8_t *out);
+
 /* ---- element-wise field kernels (device buffers); field: 0 = Fr, 1 = Fq ------------------------------------
  * op: 0 add, 1 sub, 2 mul (binary);  unary op: 0 invert (0 -> 0), 1 canonical->Montgomery, 2 Montgomery->canonical,
  * 3 square, 4 negate.  These back Polynomial +,-,* and the unit tests of the device arithmetic.                  */

@@ -13,6 +13,11 @@ use std::os::raw::{c_char, c_void};
 #[repr(C)] #[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
 pub struct zkb_check_record { pub kind: u32, pub index: u32, pub sub: u32, pub row: u32 }
 
+/// outcome of zkb_g1_decode: first bad index (u64::MAX when none), number of bad points, reason of the first (1 flag bits, 2 >= q,
+/// 3 not on the curve)
+#[repr(C)] #[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct zkb_decode_report { pub first_bad: u64, pub count: u64, pub reason: u32, pub reserved: u32 }
+
 /// create_proof's generic `T: TranscriptWrite` as four C callbacks (see gpu/transcript.rs)
 #[repr(C)]
 pub struct zkb_transcript_vtable {
@@ -40,6 +45,12 @@ extern "C" {
     pub fn zkb_srs_read(srs: *mut zkb_srs, basis: i32, out_host: *mut u64) -> i32;
     pub fn zkb_srs_commit_host(srs: *mut zkb_srs, basis: i32, scalars: *const u64, n: u64, out_affine: *mut u64, out_compressed: *mut u8) -> i32;
     pub fn zkb_srs_destroy(srs: *mut zkb_srs) -> i32;
+    // ParamsKZG::read_custom / write_custom points (format: 0 Processed, 1 RawBytes, 2 RawBytesUnchecked)
+    pub fn zkb_g1_decode(ctx: *mut zkb_ctx, format: i32, input: *const u8, n: u64, out_affine: *mut u64, rep: *mut zkb_decode_report,
+                         stream: *mut c_void) -> i32;
+    pub fn zkb_g1_encode(ctx: *mut zkb_ctx, format: i32, in_affine: *const u64, n: u64, out: *mut u8, stream: *mut c_void) -> i32;
+    pub fn zkb_g2_decode_host(format: i32, input: *const u8, out: *mut u64, status: *mut i32) -> i32;
+    pub fn zkb_g2_encode_host(format: i32, input: *const u64, out: *mut u8) -> i32;
     // keygen / proving key
     pub fn zkb_csf_validate(csf: *const u32, csf_words: u64) -> i32;
     pub fn zkb_keygen_pk(ctx: *mut zkb_ctx, csf: *const u32, csf_words: u64, fixed: *const *const u64, copies: *const u32, n_copies: u64,
