@@ -199,3 +199,13 @@ def test_super_circuit_standin(monkeypatch, capfd):
     groups = traced_groups(capfd.readouterr().err)
     assert sorted(groups) == [1, 2, 4, 8]
     assert groups[4] > groups[8]      # the condition gates (degree 5) outnumber the degree-9 set products and lookups
+
+
+@pytest.mark.parametrize("case", [test_extended_domain_of_two, test_extended_domain_of_four, test_degrees_two_to_nine_with_a_run_across_groups,
+                                  test_gaps_in_y_around_a_folded_run], ids=lambda f: f.__name__[len("test_"):])
+def test_without_coset_cache(case, monkeypatch, capfd):
+    """the proofs above, which run with the pk's coset cache of fixed, sigma, X, l_0, l_last and l_blind, made again with the cache off
+    (ZKB_COSET_CACHE_GB=0, read when the pk is built): every coset part then transforms those polynomials itself, and the bytes and
+    groups must be the same"""
+    monkeypatch.setenv("ZKB_COSET_CACHE_GB", "0")
+    case(monkeypatch, capfd)

@@ -97,6 +97,74 @@ static bool parse_csf(const uint32_t *w, uint64_t nw, Csf &c) {
     return true;
 }
 
+// parse a CSF blob and check it: node references point backwards, every column / challenge / constant index is in range
+static int32_t load_csf(const uint32_t *csf, uint64_t csf_words, Csf &c) {
+    ZKB_ARG(csf != nullptr);
+    if (!parse_csf(csf, csf_words, c)) return ZKB_ERR_ARG;
+    for (size_t i = 0; i < c.nodes.size(); ++i) {
+        const auto &nd = c.nodes[i];
+        bool ok = true;
+        switch (nd[0]) {
+        case N_CONST: ok = nd[1] < c.consts.size(); break;
+        case N_FIXED: ok = nd[1] < c.nf; break;
+        case N_ADVICE: ok = nd[1] < c.na; break;
+        case N_INSTANCE: ok = nd[1] < c.ni; break;
+        case N_CHALLENGE: ok = nd[1] < c.nch; break;
+        case N_NEG: ok = nd[1] < i; break;
+        case N_ADD: case N_MUL: ok = nd[1] < i && nd[2] < i; break;
+        case N_SCALED: ok = nd[1] < i && nd[2] < c.consts.size(); break;
+        }
+        if (!ok) { set_error("CSF: node %zu has an out-of-range operand", i); return ZKB_ERR_ARG; }
+    }
+    auto in_nodes = [&](uint32_t v) { return v < c.nodes.size(); };
+    for (auto g : c.gates) if (!in_nodes(g)) { set_error("CSF: gate references a missing node"); return ZKB_ERR_ARG; }
+    for (auto &lk : c.lookups) {
+        if (lk.inputs.empty() || lk.table.empty()) { set_error("CSF: empty lookup"); return ZKB_ERR_ARG; }
+        for (auto &inp : lk.inputs) for (auto v : inp) if (!in_nodes(v)) { set_error("CSF: lookup references a missing node"); return ZKB_ERR_ARG; }
+        for (auto v : lk.table) if (!in_nodes(v)) { set_error("CSF: lookup references a missing node"); return ZKB_ERR_ARG; }
+    }
+    for (auto &pc : c.perm) {
+        const uint32_t lim = pc[0] == N_FIXED ? c.nf : pc[0] == N_ADVICE ? c.na : pc[0] == N_INSTANCE ? c.ni : 0;
+        if (pc[1] >= lim) { set_error("CSF: permutation column out of range"); return ZKB_ERR_ARG; }
+    }
+    // queries: column in range, rotation representable in the interpreter's 16-bit field (also for expression nodes)
+    auto chkq = [&](const std::vector<std::array<int32_t, 2>> &q, uint32_t lim, const char *what) {
+        for (auto &e : q) {
+            if (e[0] < 0 || (uint32_t)e[0] >= lim) { set_error("CSF: %s query references column %d of %u", what, e[0], lim); return false; }
+            if (e[1] < -32767 || e[1] > 32767) { set_error("CSF: %s query rotation %d does not fit 16 bits", what, e[1]); return false; }
+        }
+        return true;
+    };
+    if (!chkq(c.advq, c.na, "advice") || !chkq(c.fixq, c.nf, "fixed") || !chkq(c.instq, c.ni, "instance")) return ZKB_ERR_ARG;
+    for (auto &nd : c.nodes) {
+        if (nd[0] == N_FIXED || nd[0] == N_ADVICE || nd[0] == N_INSTANCE) {
+            const int32_t rot = (int32_t)nd[2];
+            if (rot < -32767 || rot > 32767) { set_error("CSF: node rotation %d does not fit 16 bits", rot); return ZKB_ERR_ARG; }
+        }
+    }
+    if ((uint64_t)c.nf + c.na + c.ni + c.perm.size() + 1 >= 65536) { set_error("CSF: more than 65535 column slots"); return ZKB_ERR_ARG; }
+    for (uint32_t ph : c.adv_phase) if (ph >= c.nphases) { set_error("CSF: advice phase out of range"); return ZKB_ERR_ARG; }
+    for (uint32_t ph : c.ch_phase) if (ph >= c.nphases) { set_error("CSF: challenge phase out of range"); return ZKB_ERR_ARG; }
+    return ZKB_OK;
+}
+
+// The column slots of the interpreter's tables, in the one order every table uses:
+//   [fixed | advice | instance | sigma | X | l_0 | l_last | l_blind | z | phi | m]
+// The callers of the interpreter entry points pass the prefix [fixed | advice | instance].  A proof's value-domain table (lookup
+// compression, permutation products) is the prefix up to X, with X = omega^i; its quotient table is all of it on a coset part, with
+// X = the identity polynomial.  Fixed, sigma, X, l_0, l_last and l_blind do not depend on the proof: the pk caches their coset values.
+struct SlotMap {
+    uint32_t fixed0 = 0, advice0 = 0, instance0 = 0, sigma0 = 0, x = 0, l0 = 0, l_last = 0, l_blind = 0, z0 = 0, phi0 = 0, m0 = 0, slots = 0;
+    SlotMap() = default;
+    SlotMap(const Csf &cs, uint32_t nsets)
+        : advice0(cs.nf), instance0(advice0 + cs.na), sigma0(instance0 + cs.ni), x(sigma0 + (uint32_t)cs.perm.size()), l0(x + 1), l_last(x + 2),
+          l_blind(x + 3), z0(x + 4), phi0(z0 + nsets), m0(phi0 + (uint32_t)cs.lookups.size()), slots(m0 + (uint32_t)cs.lookups.size()) {}
+    // slot of a permutation column (kind, index)
+    uint32_t perm(const std::array<uint32_t, 2> &c) const { return c[0] == N_FIXED ? fixed0 + c[1] : c[0] == N_ADVICE ? advice0 + c[1] : instance0 + c[1]; }
+};
+// t[first + i] = cols[i]
+static void put_columns(std::vector<Fr *> &t, uint32_t first, const std::vector<Fr *> &cols) { std::copy(cols.begin(), cols.end(), t.begin() + first); }
+
 // ---------------------------------------------------------------------------------------------------------- small kernels
 __global__ void set_one_kernel(Fr *a, uint64_t idx) { fp_store(a + idx, Fr::one()); }
 __global__ void fill_range_one_kernel(Fr *a, uint64_t from, uint64_t to) {
@@ -150,40 +218,37 @@ __global__ void m_insert_kernel(const Fr *__restrict__ t, uint32_t usable, uint3
         h = (h + 1) & mask;
     }
 }
+constexpr uint32_t NOT_IN_TABLE = 0xffffffffu;
+// the table row holding input row i's value, or NOT_IN_TABLE
+__device__ __forceinline__ uint32_t m_probe(const Fr *__restrict__ f, uint32_t i, const Fr *__restrict__ t, const uint32_t *__restrict__ slots,
+                                            uint32_t mask) {
+    const Fr key = fp_load(f + i);
+    uint32_t h = key_hash(key) & mask;
+    while (true) {
+        const uint32_t s = slots[h];
+        if (s == 0) return NOT_IN_TABLE;
+        if (fp_load(t + (s - 1)) == key) return s - 1;
+        h = (h + 1) & mask;
+    }
+}
 __global__ void m_count_kernel(const Fr *__restrict__ f, const Fr *__restrict__ t, uint32_t usable, const uint32_t *__restrict__ slots,
                                uint32_t mask, uint32_t *counts, int *err) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    uint32_t target = 0xffffffffu;
+    uint32_t target = NOT_IN_TABLE;
     if (i < usable) {
-        const Fr key = fp_load(f + i);
-        uint32_t h = key_hash(key) & mask;
-        while (true) {
-            const uint32_t s = slots[h];
-            if (s == 0) { atomicExch(err, 1); break; }  // input not in table: unsatisfied lookup
-            if (fp_load(t + (s - 1)) == key) { target = s - 1; break; }
-            h = (h + 1) & mask;
-        }
+        target = m_probe(f, i, t, slots, mask);
+        if (target == NOT_IN_TABLE) atomicExch(err, 1);  // input not in table: unsatisfied lookup
     }
     // most rows of a zkEVM lookup hit the same few table rows (selector off -> the all-zero row): aggregate per warp
     const uint32_t peers = __match_any_sync(0xffffffffu, target);
-    if (target != 0xffffffffu && (threadIdx.x & 31) == (uint32_t)(__ffs(peers) - 1)) atomicAdd(&counts[target], (uint32_t)__popc(peers));
+    if (target != NOT_IN_TABLE && (threadIdx.x & 31) == (uint32_t)(__ffs(peers) - 1)) atomicAdd(&counts[target], (uint32_t)__popc(peers));
 }
 // witness check: the same probe as m_count_kernel, but one bit per row (word i / 32 by __ballot_sync, one writer per word) saying
 // "input row i < usable is not in the table"; launched over all words of the bitmap, rows >= usable vote 0
 __global__ void m_member_kernel(const Fr *__restrict__ f, const Fr *__restrict__ t, uint32_t usable, const uint32_t *__restrict__ slots,
                                 uint32_t mask, uint32_t *__restrict__ bits, uint32_t words) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    bool missing = false;
-    if (i < usable) {
-        const Fr key = fp_load(f + i);
-        uint32_t h = key_hash(key) & mask;
-        while (true) {
-            const uint32_t s = slots[h];
-            if (s == 0) { missing = true; break; }
-            if (fp_load(t + (s - 1)) == key) break;
-            h = (h + 1) & mask;
-        }
-    }
+    const bool missing = i < usable && m_probe(f, i, t, slots, mask) == NOT_IN_TABLE;
     const uint32_t b = __ballot_sync(0xffffffffu, missing);
     if ((threadIdx.x & 31) == 0 && (i >> 5) < words) bits[i >> 5] = b;
 }
@@ -215,6 +280,7 @@ using namespace zkb;
 struct zkb_pk {
     zkb_ctx *ctx = nullptr;
     Csf cs;
+    SlotMap sm;
     uint32_t k = 0, ext_k = 0, E = 0, qdeg = 0, chunk = 0, nsets = 0;
     uint64_t n = 0, N = 0;
     Fr omega, omega_inv, ext_omega, ext_omega_inv, n_inv, N_inv, zeta;
@@ -224,8 +290,9 @@ struct zkb_pk {
     Fr *l0_poly = nullptr, *llast_poly = nullptr, *lblind_poly = nullptr, *xid_poly = nullptr, *omega_pows = nullptr;
     zkb_srs *srs = nullptr;       // shared ParamsKZG handle (owned when the pk was made by the legacy zkb_pk_create)
     bool owns_srs = false;
-    // coset evaluations of the proof-independent polynomials (fixed, sigma, l_0, l_last, l_blind, X) for every coset part,
-    // like upstream's pk.fixed_cosets / permutation cosets / l0 / l_last / l_active_row: [part][poly] -> n elements
+    // coset evaluations of the proof-independent polynomials (fixed, sigma, X, l_0, l_last, l_blind) for every coset part, like
+    // upstream's pk.fixed_cosets / permutation cosets / l0 / l_last / l_active_row: [part][slot] -> n elements, null for the other
+    // slots; empty when the cache is off
     std::vector<std::vector<Fr *>> coset_cache;
     ~zkb_pk() {
         if (owns_srs && srs) zkb_srs_destroy(srs);
@@ -511,13 +578,6 @@ static int32_t lincomb(zkb_pk *pk, DevPool &pool, const std::vector<Fr *> &polys
     return lincomb_device(pk->ctx, d_p, d_c, (uint32_t)polys.size(), pk->n, out, accumulate, st);
 }
 
-// column slots common to the value-domain and the coset-domain tables: [fixed | advice | instance | sigma | ...]
-struct SlotMap {
-    uint32_t fixed0, advice0, instance0, sigma0;
-    explicit SlotMap(const Csf &cs) : fixed0(0), advice0(cs.nf), instance0(cs.nf + cs.na), sigma0(cs.nf + cs.na + cs.ni) {}
-    // slot of a permutation column (kind, index)
-    uint32_t perm(const std::array<uint32_t, 2> &c) const { return c[0] == N_FIXED ? fixed0 + c[1] : c[0] == N_ADVICE ? advice0 + c[1] : instance0 + c[1]; }
-};
 // translate CSF nodes into ExprBuilder nodes
 static uint32_t translate(const Csf &cs, uint32_t node, ExprBuilder &eb, const SlotMap &sm, const std::vector<Fr> &challenges, std::vector<int64_t> &memo) {
     if (memo[node] >= 0) return (uint32_t)memo[node];
@@ -544,23 +604,74 @@ static uint32_t compress_exprs(const Csf &cs, const std::vector<uint32_t> &exprs
     for (size_t i = 1; i < exprs.size(); ++i) acc = eb.add(eb.mul(acc, eb.constant(theta)), translate(cs, exprs[i], eb, sm, ch, memo));
     return acc;
 }
+// lookup l's compressed input sets into f[j] and its compressed table into t, over the 2^k rows of the d_cols table
+static int32_t lookup_compress(zkb_ctx *ctx, const Csf &cs, size_t l, const SlotMap &sm, const std::vector<Fr> &ch, const Fr &theta, DevPool &pool,
+                               const Fr *const *d_cols, std::vector<Fr *> f, Fr *t, cudaStream_t st) {
+    const CsfLookup &lk = cs.lookups[l];
+    ExprBuilder eb;
+    std::vector<int64_t> memo(cs.nodes.size(), -1);
+    std::vector<uint32_t> roots;
+    for (auto &inp : lk.inputs) roots.push_back(compress_exprs(cs, inp, eb, sm, ch, memo, theta));
+    roots.push_back(compress_exprs(cs, lk.table, eb, sm, ch, memo, theta));
+    f.push_back(t);
+    return run_store_program(ctx, cs.k, pool, eb, roots, f, d_cols, "lookup " + std::to_string(l), st);
+}
+// the hash set of table t's usable rows that m_count_kernel / m_member_kernel probe: the smallest power of two >= 2 usable slots,
+// cleared, then m_insert_kernel.  `slots` is allocated when null and otherwise reused (its size depends on `usable` only).
+static int32_t table_hash_set(zkb_ctx *ctx, DevPool &pool, const Fr *t, uint32_t usable, uint32_t *&slots, uint32_t &mask, cudaStream_t st) {
+    uint32_t tsize = 1;
+    while (tsize < 2 * usable) tsize <<= 1;
+    if (!slots) ZKB_TRY(pool.alloc((size_t)tsize * 4, (void **)&slots));
+    mask = tsize - 1;
+    ZKB_CUDA(cudaMemsetAsync(slots, 0, (size_t)tsize * 4, st));
+    if (usable) {   // the witness check takes circuits too small to have usable rows
+        m_insert_kernel<<<(usable + 255) / 256, 256, 0, st>>>(t, usable, slots, mask);
+        ctx->launches++;
+    }
+    return ZKB_OK;
+}
+
+constexpr uint32_t NO_NODE = 0xffffffffu;
+// permutation/prover.rs: the factors of set si over its columns j, multiplied left to right onto num (v_j + beta delta^j X + gamma) and
+// den (v_j + beta sigma_j + gamma); a product given as NO_NODE starts from its first factor.  X is slot sm.x in both domains.
+static void perm_set_products(const Csf &cs, const SlotMap &sm, uint32_t chunk, uint32_t si, const Fr &beta, const Fr &gamma, ExprBuilder &eb,
+                              uint32_t &num, uint32_t &den) {
+    const Fr delta = perm_delta();
+    Fr delta_pow = fp_pow_u64(delta, (uint64_t)si * chunk);
+    for (uint32_t j = si * chunk; j < std::min<size_t>((si + 1) * chunk, cs.perm.size()); ++j) {
+        const uint32_t v = eb.col(sm.perm(cs.perm[j]), 0);
+        const uint32_t dterm = eb.add(eb.add(v, eb.mul(eb.col(sm.sigma0 + j, 0), eb.constant(beta))), eb.constant(gamma));
+        const uint32_t nterm = eb.add(eb.add(v, eb.mul(eb.col(sm.x, 0), eb.constant(fp_mul(beta, delta_pow)))), eb.constant(gamma));
+        den = den == NO_NODE ? dterm : eb.mul(den, dterm);
+        num = num == NO_NODE ? nterm : eb.mul(num, nterm);
+        delta_pow = fp_mul(delta_pow, delta);
+    }
+}
 
 }  // namespace zkb
 
 // ================================================================================================ C ABI: proving key
-// Builds the device-resident proving key.  sigma columns come either from the host (sigma_values) or are already on the
-// device (sigma_dev, keygen path).  The SRS handle is shared, not copied.
-static int32_t pk_build(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, const uint64_t *const *fixed_values, const uint64_t *const *sigma_values,
+// the quotient table's proof-independent slots in coefficient form, null elsewhere
+static std::vector<Fr *> pk_quotient_polys(const zkb_pk *pk) {
+    const SlotMap &sm = pk->sm;
+    std::vector<Fr *> t(sm.slots, nullptr);
+    put_columns(t, sm.fixed0, pk->fixed_polys);
+    put_columns(t, sm.sigma0, pk->sigma_polys);
+    t[sm.x] = pk->xid_poly; t[sm.l0] = pk->l0_poly; t[sm.l_last] = pk->llast_poly; t[sm.l_blind] = pk->lblind_poly;
+    return t;
+}
+
+// Builds the device-resident proving key of a loaded CSF.  sigma columns come either from the host (sigma_values) or are already on
+// the device (sigma_dev, keygen path).  The SRS handle is shared, not copied.
+static int32_t pk_build(zkb_ctx *ctx, Csf &&csf, const uint64_t *const *fixed_values, const uint64_t *const *sigma_values,
                         const std::vector<Fr *> *sigma_dev, zkb_srs *srs, bool owns_srs, zkb_pk **out) {
-    ZKB_ARG(ctx && csf && srs && out);
     ZKB_CUDA(cudaSetDevice(ctx->device));
     std::unique_ptr<zkb_pk> pk(new zkb_pk());
     pk->ctx = ctx;
     pk->pool.ctx = ctx;
     pk->srs = srs;
     pk->owns_srs = owns_srs;
-    ZKB_TRY(zkb_csf_validate(csf, csf_words));
-    if (!parse_csf(csf, csf_words, pk->cs)) return ZKB_ERR_ARG;
+    pk->cs = std::move(csf);
     const Csf &cs = pk->cs;
     ZKB_ARG((cs.nf == 0 || fixed_values) && (cs.perm.empty() || sigma_values || sigma_dev));
     if (srs->ctx != ctx || srs->k != cs.k) { set_error("the SRS handle is for k = %u on another context or size (circuit k = %u): downsize it first", srs->k, cs.k); return ZKB_ERR_ARG; }
@@ -577,6 +688,7 @@ static int32_t pk_build(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, c
     pk->E = (uint32_t)(pk->N / n);
     pk->chunk = cs.d - 2;
     pk->nsets = (uint32_t)((cs.perm.size() + pk->chunk - 1) / pk->chunk);
+    pk->sm = SlotMap(cs, pk->nsets);
     pk->ext_omega = host_root_of_unity(pk->ext_k);
     pk->omega = pk->ext_omega;
     for (uint32_t i = cs.k; i < pk->ext_k; ++i) pk->omega = fp_sqr(pk->omega);
@@ -626,20 +738,18 @@ static int32_t pk_build(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, c
     {
         // cache the coset evaluations of the static polynomials unless that would take more than ZKB_COSET_CACHE_GB (default: a
         // quarter of the device memory, 20 GB on an 80 GB H100 -- the rest holds the proving session's columns and coset parts)
-        std::vector<Fr *> stat;
-        for (auto q : pk->fixed_polys) stat.push_back(q);
-        for (auto q : pk->sigma_polys) stat.push_back(q);
-        stat.push_back(pk->l0_poly); stat.push_back(pk->llast_poly); stat.push_back(pk->lblind_poly); stat.push_back(pk->xid_poly);
+        const std::vector<Fr *> stat = pk_quotient_polys(pk.get());
+        const size_t nstat = stat.size() - std::count(stat.begin(), stat.end(), nullptr);
         const char *env = getenv("ZKB_COSET_CACHE_GB");
         const double budget = env ? atof(env) * 1e9 : 0.25 * (double)ctx->mem_bytes;
-        if ((double)stat.size() * pk->N * sizeof(Fr) <= budget) {
+        if ((double)nstat * pk->N * sizeof(Fr) <= budget) {
             Fr *pows = nullptr;
             ZKB_TRY(pk->pool.fr(n, &pows));
-            pk->coset_cache.resize(pk->E);
+            pk->coset_cache.assign(pk->E, std::vector<Fr *>(stat.size(), nullptr));
             for (uint32_t j = 0; j < pk->E; ++j) {
                 ZKB_TRY(fr_powers_device(ctx, pk->coset_gen(j), n, pows, st));
-                pk->coset_cache[j].resize(stat.size());
                 for (size_t i = 0; i < stat.size(); ++i) {
+                    if (!stat[i]) continue;
                     ZKB_TRY(pk->pool.fr(n, &pk->coset_cache[j][i]));
                     ZKB_TRY(ntt_fr_device(ctx, stat[i], pk->coset_cache[j][i], cs.k, pk->omega, nullptr, 0, pows, st));
                 }
@@ -655,16 +765,20 @@ extern "C" int32_t zkb_pk_create(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf
                                  const uint64_t *const *sigma_values, const uint64_t *g, const uint64_t *g_lagrange, zkb_pk **out) {
     ZKB_ARG(ctx && csf && csf_words >= 18 && g && g_lagrange && out);
     ZKB_CUDA(cudaSetDevice(ctx->device));
-    ZKB_TRY(zkb_csf_validate(csf, csf_words));
+    Csf cs;
+    ZKB_TRY(load_csf(csf, csf_words, cs));
     zkb_srs *srs = nullptr;
-    ZKB_TRY(srs_create(ctx, csf[1], (const G1Affine *)g, false, (const G1Affine *)g_lagrange, false, &srs));
-    const int32_t r = pk_build(ctx, csf, csf_words, fixed_values, sigma_values, nullptr, srs, true, out);
+    ZKB_TRY(srs_create(ctx, cs.k, (const G1Affine *)g, false, (const G1Affine *)g_lagrange, false, &srs));
+    const int32_t r = pk_build(ctx, std::move(cs), fixed_values, sigma_values, nullptr, srs, true, out);
     if (r != ZKB_OK) zkb_srs_destroy(srs);
     return r;
 }
 extern "C" int32_t zkb_pk_create_with_srs(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, const uint64_t *const *fixed_values,
                                           const uint64_t *const *sigma_values, zkb_srs *srs, zkb_pk **out) {
-    return pk_build(ctx, csf, csf_words, fixed_values, sigma_values, nullptr, srs, false, out);
+    ZKB_ARG(ctx && csf && srs && out);
+    Csf cs;
+    ZKB_TRY(load_csf(csf, csf_words, cs));
+    return pk_build(ctx, std::move(cs), fixed_values, sigma_values, nullptr, srs, false, out);
 }
 
 // ---- keygen: permutation assembly + sigma columns (plonk/permutation/keygen.rs Assembly::copy, build_pk) -------------------
@@ -681,9 +795,8 @@ extern "C" int32_t zkb_keygen_pk(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf
                                  uint64_t n_copies, zkb_srs *srs, zkb_pk **out) {
     ZKB_ARG(ctx && csf && srs && out && (copies || n_copies == 0));
     ZKB_CUDA(cudaSetDevice(ctx->device));
-    ZKB_TRY(zkb_csf_validate(csf, csf_words));
     Csf cs;
-    if (!parse_csf(csf, csf_words, cs)) return ZKB_ERR_ARG;
+    ZKB_TRY(load_csf(csf, csf_words, cs));
     const uint64_t n = 1ull << cs.k;
     const size_t P = cs.perm.size();
     ZKB_ARG(P * n < (1ull << 32));
@@ -730,7 +843,7 @@ extern "C" int32_t zkb_keygen_pk(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf
     }
     ZKB_CUDA(cudaGetLastError());
     ZKB_CUDA(cudaStreamSynchronize(st));   // host vectors die at return
-    return pk_build(ctx, csf, csf_words, fixed_values, nullptr, &sig, srs, false, out);
+    return pk_build(ctx, std::move(cs), fixed_values, nullptr, &sig, srs, false, out);
 }
 // sigma column values of a proving key (n x 32 B each, Lagrange basis) back to the host: lets a caller persist / inspect keygen output
 extern "C" int32_t zkb_pk_sigma_read(zkb_pk *pk, uint32_t column, uint64_t *out_host) {
@@ -842,55 +955,8 @@ extern "C" int32_t zkb_pk_vk_bytes(zkb_pk *pk, uint8_t *out, uint64_t cap, uint6
 
 // host-only structural check of a CSF blob (no device needed)
 extern "C" int32_t zkb_csf_validate(const uint32_t *csf, uint64_t csf_words) {
-    ZKB_ARG(csf != nullptr);
     Csf c;
-    if (!parse_csf(csf, csf_words, c)) return ZKB_ERR_ARG;
-    // node references must point backwards; column / challenge / constant indices must be in range
-    for (size_t i = 0; i < c.nodes.size(); ++i) {
-        const auto &nd = c.nodes[i];
-        bool ok = true;
-        switch (nd[0]) {
-        case N_CONST: ok = nd[1] < c.consts.size(); break;
-        case N_FIXED: ok = nd[1] < c.nf; break;
-        case N_ADVICE: ok = nd[1] < c.na; break;
-        case N_INSTANCE: ok = nd[1] < c.ni; break;
-        case N_CHALLENGE: ok = nd[1] < c.nch; break;
-        case N_NEG: ok = nd[1] < i; break;
-        case N_ADD: case N_MUL: ok = nd[1] < i && nd[2] < i; break;
-        case N_SCALED: ok = nd[1] < i && nd[2] < c.consts.size(); break;
-        }
-        if (!ok) { set_error("CSF: node %zu has an out-of-range operand", i); return ZKB_ERR_ARG; }
-    }
-    auto in_nodes = [&](uint32_t v) { return v < c.nodes.size(); };
-    for (auto g : c.gates) if (!in_nodes(g)) { set_error("CSF: gate references a missing node"); return ZKB_ERR_ARG; }
-    for (auto &lk : c.lookups) {
-        if (lk.inputs.empty() || lk.table.empty()) { set_error("CSF: empty lookup"); return ZKB_ERR_ARG; }
-        for (auto &inp : lk.inputs) for (auto v : inp) if (!in_nodes(v)) { set_error("CSF: lookup references a missing node"); return ZKB_ERR_ARG; }
-        for (auto v : lk.table) if (!in_nodes(v)) { set_error("CSF: lookup references a missing node"); return ZKB_ERR_ARG; }
-    }
-    for (auto &pc : c.perm) {
-        const uint32_t lim = pc[0] == N_FIXED ? c.nf : pc[0] == N_ADVICE ? c.na : pc[0] == N_INSTANCE ? c.ni : 0;
-        if (pc[1] >= lim) { set_error("CSF: permutation column out of range"); return ZKB_ERR_ARG; }
-    }
-    // queries: column in range, rotation representable in the interpreter's 16-bit field (also for expression nodes)
-    auto chkq = [&](const std::vector<std::array<int32_t, 2>> &q, uint32_t lim, const char *what) {
-        for (auto &e : q) {
-            if (e[0] < 0 || (uint32_t)e[0] >= lim) { set_error("CSF: %s query references column %d of %u", what, e[0], lim); return false; }
-            if (e[1] < -32767 || e[1] > 32767) { set_error("CSF: %s query rotation %d does not fit 16 bits", what, e[1]); return false; }
-        }
-        return true;
-    };
-    if (!chkq(c.advq, c.na, "advice") || !chkq(c.fixq, c.nf, "fixed") || !chkq(c.instq, c.ni, "instance")) return ZKB_ERR_ARG;
-    for (auto &nd : c.nodes) {
-        if (nd[0] == N_FIXED || nd[0] == N_ADVICE || nd[0] == N_INSTANCE) {
-            const int32_t rot = (int32_t)nd[2];
-            if (rot < -32767 || rot > 32767) { set_error("CSF: node rotation %d does not fit 16 bits", rot); return ZKB_ERR_ARG; }
-        }
-    }
-    if ((uint64_t)c.nf + c.na + c.ni + c.perm.size() + 1 >= 65536) { set_error("CSF: more than 65535 column slots"); return ZKB_ERR_ARG; }
-    for (uint32_t ph : c.adv_phase) if (ph >= c.nphases) { set_error("CSF: advice phase out of range"); return ZKB_ERR_ARG; }
-    for (uint32_t ph : c.ch_phase) if (ph >= c.nphases) { set_error("CSF: challenge phase out of range"); return ZKB_ERR_ARG; }
-    return ZKB_OK;
+    return load_csf(csf, csf_words, c);
 }
 
 extern "C" int32_t zkb_pk_destroy(zkb_pk *pk) {
@@ -1079,7 +1145,7 @@ struct OpenQuery {
 // what one stage of the proof hands to a later one
 struct ProofState {
     Fr theta, beta, gamma, y, x;
-    Fr **d_vcols = nullptr;                  // value-domain column table: [fixed | advice | instance | sigma | omega_pows]
+    Fr **d_vcols = nullptr;                  // value-domain column table: the SlotMap prefix up to X (omega_pows)
     std::vector<std::vector<Fr *>> lk_f;     // compressed inputs per lookup / input set
     std::vector<Fr *> lk_t, lk_m;            // compressed table, multiplicities per lookup
     std::vector<Fr *> zs, phis;              // permutation grand products per set, lookup grand sums per lookup
@@ -1105,53 +1171,29 @@ static int32_t lookup_prepare(zkb_session *s, ProofState &ps) {
     cudaStream_t st = ctx->stream;
     DevPool &pool = s->pool;
     ps.theta = tr_squeeze(s);
-    const SlotMap sm(cs);
-    std::vector<Fr *> vcols;
-    for (auto p : pk->fixed_values) vcols.push_back(p);
-    for (auto p : s->adv_values) vcols.push_back(p);
-    for (auto p : s->inst_values) vcols.push_back(p);
-    for (auto p : pk->sigma_values) vcols.push_back(p);
-    vcols.push_back(pk->omega_pows);
-    ZKB_TRY(upload_table(pool, vcols, &ps.d_vcols, st));
-
     ps.lk_f.resize(nl);
     ps.lk_t.resize(nl);
     const Deal deal(ctx, nl);
     Fr *m_slab = nullptr;
     ZKB_TRY(dealt_columns(pool, deal, n, ps.lk_m, &m_slab));
+    uint32_t *slots = nullptr, mask = 0;
     uint64_t lookup_errors = 0;
     for (size_t l = 0; l < nl; ++l) {
         if (!deal.mine(l)) continue;
-        const CsfLookup &lk = cs.lookups[l];
-        ExprBuilder eb;
-        std::vector<int64_t> memo(cs.nodes.size(), -1);
-        std::vector<uint32_t> roots;
-        for (size_t j = 0; j < lk.inputs.size(); ++j) {
-            Fr *a;
-            ZKB_TRY(pool.fr(n, &a));
-            ps.lk_f[l].push_back(a);
-            roots.push_back(compress_exprs(cs, lk.inputs[j], eb, sm, s->challenges, memo, ps.theta));
-        }
+        const size_t ns = cs.lookups[l].inputs.size();
+        ps.lk_f[l].resize(ns);
+        for (auto &f : ps.lk_f[l]) ZKB_TRY(pool.fr(n, &f));
         ZKB_TRY(pool.fr(n, &ps.lk_t[l]));
-        roots.push_back(compress_exprs(cs, lk.table, eb, sm, s->challenges, memo, ps.theta));
-        std::vector<Fr *> outs = ps.lk_f[l];
-        outs.push_back(ps.lk_t[l]);
-        ZKB_TRY(run_store_program(pk->ctx, pk->k, pool, eb, roots, outs, ps.d_vcols, "lookup " + std::to_string(l), st));
+        ZKB_TRY(lookup_compress(ctx, cs, l, pk->sm, s->challenges, ps.theta, pool, ps.d_vcols, ps.lk_f[l], ps.lk_t[l], st));
         // multiplicities over the usable rows
-        uint32_t tsize = 1;
-        while (tsize < 2 * usable) tsize <<= 1;
-        uint32_t *slots = nullptr, *counts = nullptr;
-        int *d_err = nullptr;
-        ZKB_TRY(pool.alloc((size_t)tsize * 4, (void **)&slots));
+        ZKB_TRY(table_hash_set(ctx, pool, ps.lk_t[l], usable, slots, mask, st));
+        uint32_t *counts = nullptr;
         ZKB_TRY(pool.alloc((size_t)n * 4 + 16, (void **)&counts));
-        d_err = (int *)(counts + n);
-        ZKB_CUDA(cudaMemsetAsync(slots, 0, (size_t)tsize * 4, st));
+        int *d_err = (int *)(counts + n);
         ZKB_CUDA(cudaMemsetAsync(counts, 0, (size_t)n * 4 + 16, st));
-        const unsigned ub = (usable + 255) / 256;
-        m_insert_kernel<<<ub, 256, 0, st>>>(ps.lk_t[l], usable, slots, tsize - 1);
-        for (size_t j = 0; j < lk.inputs.size(); ++j) m_count_kernel<<<ub, 256, 0, st>>>(ps.lk_f[l][j], ps.lk_t[l], usable, slots, tsize - 1, counts, d_err);
+        for (size_t j = 0; j < ns; ++j) m_count_kernel<<<(usable + 255) / 256, 256, 0, st>>>(ps.lk_f[l][j], ps.lk_t[l], usable, slots, mask, counts, d_err);
         counts_to_fr_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(counts, (uint32_t)n, ps.lk_m[l]);
-        ctx->launches += 2 + lk.inputs.size();
+        ctx->launches += 1 + ns;
         int herr = 0;
         ZKB_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, st));
         ZKB_CUDA(cudaStreamSynchronize(st));
@@ -1190,9 +1232,6 @@ static int32_t permutation_commit(zkb_session *s, ProofState &ps, const uint64_t
     DevPool &pool = s->pool;
     ps.beta = tr_squeeze(s);
     ps.gamma = tr_squeeze(s);
-    const SlotMap sm(cs);
-    const uint32_t v_omega = sm.sigma0 + (uint32_t)cs.perm.size();
-    const Fr delta = perm_delta();
     // Multi-GPU: the sets are dealt.  Upstream chains them (z_i[0] = last value of z_{i-1}), which is sequential; here every set is
     // scanned from 1 and rescaled afterwards by c_i = product of the previous sets' last values -- the same field elements
     // (z_i = c_i * z'_i row by row), with only the nsets last values crossing the ranks before the columns are gathered.
@@ -1210,18 +1249,8 @@ static int32_t permutation_commit(zkb_session *s, ProofState &ps, const uint64_t
     for (uint32_t si = 0; si < pk->nsets; ++si) {
         if (!deal.mine(si)) continue;
         ExprBuilder eb;
-        uint32_t nnum = 0, nden = 0;
-        bool first = true;
-        Fr delta_pow = fp_pow_u64(delta, (uint64_t)si * pk->chunk);
-        for (uint32_t j = si * pk->chunk; j < std::min<size_t>((si + 1) * pk->chunk, cs.perm.size()); ++j) {
-            const uint32_t v = eb.col(sm.perm(cs.perm[j]), 0);
-            const uint32_t dterm = eb.add(eb.add(v, eb.mul(eb.col(sm.sigma0 + j, 0), eb.constant(ps.beta))), eb.constant(ps.gamma));
-            const uint32_t nterm = eb.add(eb.add(v, eb.mul(eb.col(v_omega, 0), eb.constant(fp_mul(ps.beta, delta_pow)))), eb.constant(ps.gamma));
-            nden = first ? dterm : eb.mul(nden, dterm);
-            nnum = first ? nterm : eb.mul(nnum, nterm);
-            first = false;
-            delta_pow = fp_mul(delta_pow, delta);
-        }
+        uint32_t nnum = NO_NODE, nden = NO_NODE;
+        perm_set_products(cs, pk->sm, pk->chunk, si, ps.beta, ps.gamma, eb, nnum, nden);
         ZKB_TRY(run_store_program(pk->ctx, pk->k, pool, eb, {nnum, nden}, {num, den}, ps.d_vcols, "permutation", st));
         ZKB_TRY(batch_invert_device(ctx, den, tmp, n, st));
         mul_arrays_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(num, tmp, den, n);  // den <- modified values
@@ -1460,25 +1489,14 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
     const Fr one = Fr::one();
     cudaStream_t st = ctx->stream;
     DevPool &pool = s->pool;
-    // coset-domain slot table: [fixed | advice | instance | sigma | z | phi | m | l0 | l_last | l_blind | X]
-    const SlotMap sm(cs);
-    std::vector<Fr *> qpolys;
-    for (auto p : pk->fixed_polys) qpolys.push_back(p);
-    for (auto p : ps.adv_polys) qpolys.push_back(p);
-    for (auto p : s->inst_polys) qpolys.push_back(p);
-    for (auto p : pk->sigma_polys) qpolys.push_back(p);
-    const uint32_t q_z0 = (uint32_t)qpolys.size();
-    for (auto p : ps.z_polys) qpolys.push_back(p);
-    const uint32_t q_phi0 = (uint32_t)qpolys.size();
-    for (auto p : ps.phi_polys) qpolys.push_back(p);
-    const uint32_t q_m0 = (uint32_t)qpolys.size();
-    for (auto p : ps.m_polys) qpolys.push_back(p);
-    const uint32_t q_l0 = (uint32_t)qpolys.size();
-    qpolys.push_back(pk->l0_poly);
-    qpolys.push_back(pk->llast_poly);
-    qpolys.push_back(pk->lblind_poly);
-    qpolys.push_back(pk->xid_poly);
-    const uint32_t q_llast = q_l0 + 1, q_lblind = q_l0 + 2, q_x = q_l0 + 3;
+    // the quotient table in coefficient form
+    const SlotMap &sm = pk->sm;
+    std::vector<Fr *> qpolys = pk_quotient_polys(pk);
+    put_columns(qpolys, sm.advice0, ps.adv_polys);
+    put_columns(qpolys, sm.instance0, s->inst_polys);
+    put_columns(qpolys, sm.z0, ps.z_polys);
+    put_columns(qpolys, sm.phi0, ps.phi_polys);
+    put_columns(qpolys, sm.m0, ps.m_polys);
     ZKB_ARG(qpolys.size() < 65536);
 
     const uint32_t E = pk->E;
@@ -1491,25 +1509,18 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
     QuotientGroups qg(qeb, ps.y, E, qpb_ptrs);
     std::vector<int64_t> memo(cs.nodes.size(), -1);
     ZKB_TRY(quotient_gates(cs, s->challenges, qg, sm, memo));
-    auto lactive = [&]() { return qeb.sub(qeb.sub(qeb.constant(one), qeb.col(q_llast, 0)), qeb.col(q_lblind, 0)); };
+    auto lactive = [&]() { return qeb.sub(qeb.sub(qeb.constant(one), qeb.col(sm.l_last, 0)), qeb.col(sm.l_blind, 0)); };
     if (pk->nsets) {
-        const uint32_t z0 = qeb.col(q_z0, 0), zl = qeb.col(q_z0 + pk->nsets - 1, 0);
-        if (!qg.scope({qeb.mul(qeb.sub(qeb.constant(one), z0), qeb.col(q_l0, 0))})) return ZKB_ERR_ARG;
-        if (!qg.scope({qeb.mul(qeb.sub(qeb.mul(zl, zl), zl), qeb.col(q_llast, 0))})) return ZKB_ERR_ARG;
+        const uint32_t z0 = qeb.col(sm.z0, 0), zl = qeb.col(sm.z0 + pk->nsets - 1, 0);
+        if (!qg.scope({qeb.mul(qeb.sub(qeb.constant(one), z0), qeb.col(sm.l0, 0))})) return ZKB_ERR_ARG;
+        if (!qg.scope({qeb.mul(qeb.sub(qeb.mul(zl, zl), zl), qeb.col(sm.l_last, 0))})) return ZKB_ERR_ARG;
         for (uint32_t i = 1; i < pk->nsets; ++i) {
-            const uint32_t t = qeb.mul(qeb.sub(qeb.col(q_z0 + i, 0), qeb.col(q_z0 + i - 1, -(int32_t)(cs.bf + 1))), qeb.col(q_l0, 0));
+            const uint32_t t = qeb.mul(qeb.sub(qeb.col(sm.z0 + i, 0), qeb.col(sm.z0 + i - 1, -(int32_t)(cs.bf + 1))), qeb.col(sm.l0, 0));
             if (!qg.scope({t})) return ZKB_ERR_ARG;
         }
-        const Fr delta = perm_delta();
-        Fr delta_pow = one;
         for (uint32_t si = 0; si < pk->nsets; ++si) {
-            uint32_t left = qeb.col(q_z0 + si, 1), right = qeb.col(q_z0 + si, 0);
-            for (uint32_t j = si * pk->chunk; j < std::min<size_t>((si + 1) * pk->chunk, cs.perm.size()); ++j) {
-                const uint32_t v = qeb.col(sm.perm(cs.perm[j]), 0);
-                left = qeb.mul(left, qeb.add(qeb.add(v, qeb.mul(qeb.col(sm.sigma0 + j, 0), qeb.constant(ps.beta))), qeb.constant(ps.gamma)));
-                right = qeb.mul(right, qeb.add(qeb.add(v, qeb.mul(qeb.col(q_x, 0), qeb.constant(fp_mul(ps.beta, delta_pow)))), qeb.constant(ps.gamma)));
-                delta_pow = fp_mul(delta_pow, delta);
-            }
+            uint32_t left = qeb.col(sm.z0 + si, 1), right = qeb.col(sm.z0 + si, 0);
+            perm_set_products(cs, sm, pk->chunk, si, ps.beta, ps.gamma, qeb, right, left);
             if (!qg.scope({qeb.mul(qeb.sub(left, right), lactive())})) { set_error("permutation: %s", qg.error.c_str()); return ZKB_ERR_ARG; }
         }
     }
@@ -1534,10 +1545,10 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
             ssum = have_sum ? qeb.add(ssum, pr) : pr;
             have_sum = true;
         }
-        const uint32_t phi = qeb.col(q_phi0 + (uint32_t)l, 0), phi_next = qeb.col(q_phi0 + (uint32_t)l, 1), m = qeb.col(q_m0 + (uint32_t)l, 0);
+        const uint32_t phi = qeb.col(sm.phi0 + (uint32_t)l, 0), phi_next = qeb.col(sm.phi0 + (uint32_t)l, 1), m = qeb.col(sm.m0 + (uint32_t)l, 0);
         const uint32_t lhs = qeb.mul(qeb.mul(tb, prod), qeb.sub(phi_next, phi));
         const uint32_t rhs = qeb.sub(qeb.mul(tb, ssum), qeb.mul(m, prod));
-        if (!qg.scope({qeb.mul(phi, qeb.col(q_l0, 0)), qeb.mul(phi, qeb.col(q_llast, 0)), qeb.mul(qeb.sub(lhs, rhs), lactive())})) {
+        if (!qg.scope({qeb.mul(phi, qeb.col(sm.l0, 0)), qeb.mul(phi, qeb.col(sm.l_last, 0)), qeb.mul(qeb.sub(lhs, rhs), lactive())})) {
             set_error("lookup %zu: %s", l, qg.error.c_str());
             return ZKB_ERR_ARG;
         }
@@ -1562,15 +1573,8 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
         qpbs[g].store_acc(0, scale_idx[g][0]);
         ZKB_TRY(upload_program(pool, qpbs[g], qeb, qdp[g], st));
     }
-    // slots served from the pk's coset cache: fixed, sigma, l0 / l_last / l_blind / X
-    const bool cached = !pk->coset_cache.empty();
-    std::vector<int> cache_idx(qpolys.size(), -1);
-    if (cached) {
-        int ci = 0;
-        for (uint32_t i = 0; i < cs.nf; ++i) cache_idx[sm.fixed0 + i] = ci++;
-        for (size_t i = 0; i < cs.perm.size(); ++i) cache_idx[sm.sigma0 + i] = ci++;
-        cache_idx[q_l0] = ci++; cache_idx[q_llast] = ci++; cache_idx[q_lblind] = ci++; cache_idx[q_x] = ci++;
-    }
+    // slots served from the pk's coset cache
+    auto cached = [&](size_t i) { return !pk->coset_cache.empty() && pk->coset_cache[0][i]; };
     // the largest group reading each slot: a polynomial outside the cache is transformed on that group's parts (a smaller group's
     // parts are a subset of them), and not at all when no constraint reads it
     std::vector<int> reader(qpolys.size(), -1);
@@ -1588,7 +1592,7 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
         for (uint32_t g : groups) {
             size_t instrs = 0, ntts = 0;
             for (const Instr &in : qpbs[g].code) instrs += in.op != OP_ARG;
-            for (size_t i = 0; i < qpolys.size(); ++i) ntts += cache_idx[i] < 0 && reader[i] == (int)g;
+            for (size_t i = 0; i < qpolys.size(); ++i) ntts += !cached(i) && reader[i] == (int)g;
             fprintf(stderr, "[zkb trace] quotient group m = %-2u %6u constraints %7zu instructions/row %5zu coset NTTs\n", 1u << g, qg.count[g],
                     instrs, ntts << g);
         }
@@ -1633,15 +1637,14 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
         if (!dq.mine(j)) continue;
         std::vector<Fr *> ntt_src, ntt_dst;
         for (size_t i = 0; i < qpolys.size(); ++i)
-            if (cache_idx[i] < 0 && reader[i] >= 0 && on_part((uint32_t)reader[i], j)) { ntt_src.push_back(qpolys[i]); ntt_dst.push_back(qcols[i]); }
+            if (!cached(i) && reader[i] >= 0 && on_part((uint32_t)reader[i], j)) { ntt_src.push_back(qpolys[i]); ntt_dst.push_back(qcols[i]); }
         if (!ntt_src.empty()) {
             ZKB_TRY(fr_powers_device(ctx, pk->coset_gen(j), n, pows, st));
             ZKB_TRY(ntt_many(pk, ntt_src, ntt_dst, pk->omega, nullptr, pows, st));
         }
         std::vector<Fr *> cols_j = qcols;
-        if (cached)
-            for (size_t i = 0; i < qpolys.size(); ++i)
-                if (cache_idx[i] >= 0) cols_j[i] = pk->coset_cache[j][cache_idx[i]];
+        for (size_t i = 0; i < qpolys.size(); ++i)
+            if (cached(i)) cols_j[i] = pk->coset_cache[j][i];
         ZKB_CUDA(cudaMemcpyAsync(d_qcols, cols_j.data(), cols_j.size() * sizeof(Fr *), cudaMemcpyHostToDevice, st));
         std::vector<Instr> tails(G);
         for (uint32_t g : groups) {
@@ -1935,8 +1938,18 @@ static int32_t shplonk(zkb_session *s, ProofState &ps) {
 
 // create_proof after the advice phases (plonk/prover.rs), one function per upstream stage, in transcript order
 static int32_t prove_finish_stages(zkb_session *s, const uint64_t *z_blinds, const uint64_t *phi_blinds, const uint64_t *random_poly_host) {
+    zkb_pk *pk = s->pk;
     ProofState ps;
-    StageTrace trace(s->pk->ctx->stream);
+    StageTrace trace(pk->ctx->stream);
+    // the value-domain column table of the lookup compression and the permutation products
+    const SlotMap &sm = pk->sm;
+    std::vector<Fr *> vcols(sm.x + 1);
+    put_columns(vcols, sm.fixed0, pk->fixed_values);
+    put_columns(vcols, sm.advice0, s->adv_values);
+    put_columns(vcols, sm.instance0, s->inst_values);
+    put_columns(vcols, sm.sigma0, pk->sigma_values);
+    vcols[sm.x] = pk->omega_pows;
+    ZKB_TRY(upload_table(s->pool, vcols, &ps.d_vcols, pk->ctx->stream));
     ZKB_TRY(lookup_prepare(s, ps));
     trace.mark("lookups: compress + m + commit");
     ZKB_TRY(permutation_commit(s, ps, z_blinds));
@@ -1987,15 +2000,14 @@ extern "C" int32_t zkb_prove_finish(zkb_session *s, const uint64_t *z_blinds, co
 // ================================================================================================ C ABI: constraint interpreter
 // The gates of a CSF evaluated over caller columns by the prover's own compiler (translate, ProgramBuilder, quotient_gates) and
 // interpreter (expr_run_device): the hot kernel of a proof checked row by row against a reference evaluator.
-// The gate program of zkb_expr_eval_dev / zkb_expr_program (csf already validated and parsed into cs).  Mode 0: every gate a
-// STORE root of ONE CSE scope, like the lookup compression programs.  Mode 1: the gate part of evaluate_h's quotient program,
-// then one STOREACC with `scale`.
-static int32_t gate_program(const Csf &cs, int32_t mode, const uint64_t *challenges, const uint64_t y[4], const uint64_t scale[4],
+// The gate program of zkb_expr_eval_dev / zkb_expr_program over the caller's columns, the [fixed | advice | instance] prefix of
+// SlotMap.  Mode 0: every gate a STORE root of ONE CSE scope, like the lookup compression programs.  Mode 1: the gate part of
+// evaluate_h's quotient program, then one STOREACC with `scale`.
+static int32_t gate_program(const Csf &cs, const SlotMap &sm, int32_t mode, const uint64_t *challenges, const uint64_t y[4], const uint64_t scale[4],
                             ExprBuilder &eb, ProgramBuilder &pb) {
     ZKB_ARG(cs.nch == 0 || challenges);
     std::vector<Fr> ch(cs.nch);
     for (uint32_t i = 0; i < cs.nch; ++i) memcpy(ch[i].l, challenges + 4 * i, sizeof(Fr));
-    const SlotMap sm(cs);
     std::vector<int64_t> memo(cs.nodes.size(), -1);
     if (mode == 0) {
         std::vector<ProgramBuilder::Root> roots;
@@ -2018,15 +2030,14 @@ extern "C" int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t
     ZKB_ARG(ctx && csf && columns_dev && outs_dev && (mode == 0 || mode == 1));
     ZKB_ARG(mode == 0 ? out_stride == 1 && out_offset == 0 : y && scale && out_stride >= 1);
     ZKB_CUDA(cudaSetDevice(ctx->device));
-    ZKB_TRY(zkb_csf_validate(csf, csf_words));
     Csf cs;
-    parse_csf(csf, csf_words, cs);
+    ZKB_TRY(load_csf(csf, csf_words, cs));
+    const SlotMap sm(cs, 0);
     ExprBuilder eb;
     ProgramBuilder pb(eb);
-    ZKB_TRY(gate_program(cs, mode, challenges, y, scale, eb, pb));
+    ZKB_TRY(gate_program(cs, sm, mode, challenges, y, scale, eb, pb));
     cudaStream_t st = pick_stream(ctx, stream);
-    std::vector<Fr *> cols(cs.nf + cs.na + cs.ni);
-    for (size_t i = 0; i < cols.size(); ++i) cols[i] = (Fr *)columns_dev[i];
+    const std::vector<Fr *> cols((Fr *const *)columns_dev, (Fr *const *)columns_dev + sm.sigma0);
     std::vector<Fr *> outs(mode == 0 ? cs.gates.size() : 1);
     for (size_t i = 0; i < outs.size(); ++i) outs[i] = (Fr *)outs_dev[i];
     DevPool pool;
@@ -2045,12 +2056,11 @@ extern "C" int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t
 extern "C" int32_t zkb_expr_program(const uint32_t *csf, uint64_t csf_words, int32_t mode, const uint64_t *challenges, const uint64_t y[4],
                                     const uint64_t scale[4], uint64_t *code_out, uint64_t cap, uint64_t *ncode_out, uint32_t *nregs_out) {
     ZKB_ARG(csf && ncode_out && (mode == 0 || mode == 1) && (mode == 0 || (y && scale)) && (code_out || cap == 0));
-    ZKB_TRY(zkb_csf_validate(csf, csf_words));
     Csf cs;
-    parse_csf(csf, csf_words, cs);
+    ZKB_TRY(load_csf(csf, csf_words, cs));
     ExprBuilder eb;
     ProgramBuilder pb(eb);
-    ZKB_TRY(gate_program(cs, mode, challenges, y, scale, eb, pb));
+    ZKB_TRY(gate_program(cs, SlotMap(cs, 0), mode, challenges, y, scale, eb, pb));
     static_assert(sizeof(Instr) == sizeof(uint64_t), "one program word per instruction");
     *ncode_out = pb.code.size();
     if (nregs_out) *nregs_out = (uint32_t)pb.max_regs_used;
@@ -2068,9 +2078,8 @@ extern "C" int32_t zkb_check_witness_dev(zkb_ctx *ctx, const uint32_t *csf, uint
     ZKB_ARG(ctx && csf && columns_dev && counts_out && n_records && (records_out || cap == 0) && (copies_dev || n_copies == 0));
     ZKB_ARG(n_copies < (1ull << 32));
     ZKB_CUDA(cudaSetDevice(ctx->device));
-    ZKB_TRY(zkb_csf_validate(csf, csf_words));
     Csf cs;
-    parse_csf(csf, csf_words, cs);
+    ZKB_TRY(load_csf(csf, csf_words, cs));
     if (cs.nch && !challenges) { set_error("zkb_check_witness_dev: the constraint system has %u challenges and none were given", cs.nch); return ZKB_ERR_ARG; }
     for (size_t l = 0; l < cs.lookups.size(); ++l)
         if (cs.lookups[l].table.size() > 1 && !theta) {
@@ -2084,9 +2093,8 @@ extern "C" int32_t zkb_check_witness_dev(zkb_ctx *ctx, const uint32_t *csf, uint
     cudaStream_t st = pick_stream(ctx, stream);
     const uint32_t n = 1u << cs.k, words = (n + 31) / 32;
     const uint32_t usable = n > cs.bf + 1 ? n - cs.bf - 1 : 0;
-    const SlotMap sm(cs);
-    std::vector<Fr *> cols(cs.nf + cs.na + cs.ni);
-    for (size_t i = 0; i < cols.size(); ++i) cols[i] = (Fr *)columns_dev[i];
+    const SlotMap sm(cs, 0);   // the caller's columns are its [fixed | advice | instance] prefix
+    const std::vector<Fr *> cols((Fr *const *)columns_dev, (Fr *const *)columns_dev + sm.sigma0);
     size_t nsets = 0, maxsets = 0;
     for (auto &lk : cs.lookups) { nsets += lk.inputs.size(); maxsets = std::max(maxsets, lk.inputs.size()); }
     const uint64_t copy_words = (n_copies + 31) / 32;
@@ -2119,29 +2127,14 @@ extern "C" int32_t zkb_check_witness_dev(zkb_ctx *ctx, const uint32_t *csf, uint
         ProfScope ps_(ctx, PROF_CHECK_LOOKUPS, st);
         std::vector<Fr *> bufs(maxsets + 1);
         for (auto &b : bufs) ZKB_TRY(pool.fr(n, &b));
-        uint32_t tsize = 1;
-        while (tsize < 2 * usable) tsize <<= 1;
-        uint32_t *slots = nullptr;
-        ZKB_TRY(pool.alloc((size_t)tsize * 4, (void **)&slots));
+        uint32_t *slots = nullptr, mask = 0;
         uint32_t *out = lk_bits;
         for (size_t l = 0; l < cs.lookups.size(); ++l) {
-            const CsfLookup &lk = cs.lookups[l];
-            const size_t ns = lk.inputs.size();
-            ExprBuilder eb;
-            std::vector<int64_t> memo(cs.nodes.size(), -1);
-            std::vector<uint32_t> roots;
-            for (size_t j = 0; j < ns; ++j) roots.push_back(compress_exprs(cs, lk.inputs[j], eb, sm, ch, memo, th));
-            roots.push_back(compress_exprs(cs, lk.table, eb, sm, ch, memo, th));
-            std::vector<Fr *> outs(bufs.begin(), bufs.begin() + ns);
-            outs.push_back(bufs[maxsets]);
-            ZKB_TRY(run_store_program(ctx, cs.k, pool, eb, roots, outs, d_cols, "lookup " + std::to_string(l), st));
-            ZKB_CUDA(cudaMemsetAsync(slots, 0, (size_t)tsize * 4, st));
-            if (usable) {
-                m_insert_kernel<<<(usable + 255) / 256, 256, 0, st>>>(bufs[maxsets], usable, slots, tsize - 1);
-                ctx->launches++;
-            }
+            const size_t ns = cs.lookups[l].inputs.size();
+            ZKB_TRY(lookup_compress(ctx, cs, l, sm, ch, th, pool, d_cols, std::vector<Fr *>(bufs.begin(), bufs.begin() + ns), bufs[maxsets], st));
+            ZKB_TRY(table_hash_set(ctx, pool, bufs[maxsets], usable, slots, mask, st));
             for (size_t j = 0; j < ns; ++j, out += words) {
-                m_member_kernel<<<(n + 255) / 256, 256, 0, st>>>(bufs[j], bufs[maxsets], usable, slots, tsize - 1, out, words);
+                m_member_kernel<<<(n + 255) / 256, 256, 0, st>>>(bufs[j], bufs[maxsets], usable, slots, mask, out, words);
                 ctx->launches++;
                 items.push_back({out, words, 1, (uint32_t)l, (uint32_t)j, 0, 0});
             }
