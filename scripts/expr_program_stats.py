@@ -7,7 +7,9 @@ The unfused program is rebuilt from the fused one: every column (C) or constant 
 OP_LOADCOL / OP_LOADCONST into a register that the plain form then read.  Per row it prints
   - interpreted instructions (dispatches) by opcode, and program words fetched (a fused form with two C / K operands is two words);
   - register-file accesses: an access moves one 32-byte field element, two 16-byte LDS / STS in the shared-memory builds;
-  - global field-element loads: columns, constants (including the y powers of HORNER / FOLD and STOREACC's scale).
+  - global field-element loads: columns, constants (including the y powers of HORNER / FOLD and STOREACC's scale);
+  - Montgomery products and reductions: MUL, HORNER, HORNER2 and STOREACC are one product and one reduction each; FOLD
+    (acc * y^r + f * acc2) and the merged HORNER_M / HORNER2_M (acc * y + a * b) two products with one reduction.
 usage: python scripts/expr_program_stats.py [--shape super|keccak] [--k K] [--mode 0|1] [--json]"""
 import argparse
 import collections
@@ -23,7 +25,7 @@ import numpy as np
 
 # opcodes of csrc/expr.cuh
 BASE = {0: "LOADCOL", 1: "LOADCONST", 2: "ADD", 3: "SUB", 4: "MUL", 5: "NEG", 6: "HORNER", 7: "STORE", 8: "STOREACC",
-        9: "CLEARACC", 10: "HORNER2", 11: "FOLD", 12: "FLAG"}
+        9: "CLEARACC", 10: "HORNER2", 11: "FOLD", 12: "FLAG", 43: "HORNER_M", 44: "HORNER2_M"}
 ARG = 13
 FORMS = ["RC", "CR", "RK", "KR", "CC", "CK", "KC"]
 FUSED = {16 + f: ("ADD", FORMS[f]) for f in range(7)}
@@ -64,6 +66,15 @@ def counts(ops, words):
             continue
         name = BASE[o]
         fused[name] += 1
+        if name in ("HORNER_M", "HORNER2_M"):        # merged: unfused it is a MUL (2 reads, 1 write) and the root (1 read)
+            plain["MUL"] += 1
+            plain[name[:-2]] += 1
+            rf["fused"][0] += 2
+            rf["plain"][0] += 3
+            rf["plain"][1] += 1
+            loads["fused"] += 1
+            loads["plain"] += 1
+            continue
         plain[name] += 1
         reads = {"ADD": 2, "SUB": 2, "MUL": 2, "NEG": 1, "HORNER": 1, "HORNER2": 1, "FOLD": 1, "STORE": 1, "FLAG": 1}.get(name, 0)
         writes = 1 if name in ("LOADCOL", "LOADCONST", "ADD", "SUB", "MUL", "NEG") else 0
@@ -72,7 +83,16 @@ def counts(ops, words):
             rf[key][0] += reads
             rf[key][1] += writes
             loads[key] += gl
-    return {"fused": {"dispatches": sum(fused.values()), "words": words, "by_op": dict(sorted(fused.items())),
+    # Montgomery multiplies per row: (products, reductions) of the program as it runs
+    cost = {"MUL": (1, 1), "HORNER": (1, 1), "HORNER2": (1, 1), "STOREACC": (1, 1), "FOLD": (2, 1), "HORNER_M": (2, 1),
+            "HORNER2_M": (2, 1)}
+    by = collections.Counter()
+    for k, v in fused.items():
+        by[k.split("_")[0] if k.split("_")[-1] in FORMS or k.endswith("_C") else k] += v
+    products = sum(cost.get(k, (0, 0))[0] * v for k, v in by.items())
+    reductions = sum(cost.get(k, (0, 0))[1] * v for k, v in by.items())
+    return {"products": products, "reductions": reductions,
+            "fused": {"dispatches": sum(fused.values()), "words": words, "by_op": dict(sorted(fused.items())),
                       "regfile_reads": rf["fused"][0], "regfile_writes": rf["fused"][1], "global_loads": loads["fused"]},
             "unfused": {"dispatches": sum(plain.values()), "words": sum(plain.values()), "by_op": dict(sorted(plain.items())),
                         "regfile_reads": rf["plain"][0], "regfile_writes": rf["plain"][1], "global_loads": loads["plain"]}}
@@ -107,6 +127,7 @@ def main():
     print(f"{'':24}{'unfused':>10}{'fused':>10}")
     for key in ("dispatches", "words", "regfile_reads", "regfile_writes", "global_loads"):
         print(f"{key:24}{p[key]:>10}{f[key]:>10}")
+    print(f"Montgomery products {res['products']}, reductions {res['reductions']} per row")
     print("dispatches by opcode:")
     for name in sorted(set(f["by_op"]) | set(p["by_op"])):
         print(f"  {name:22}{p['by_op'].get(name, 0):>10}{f['by_op'].get(name, 0):>10}")

@@ -57,6 +57,7 @@ struct FlagLaunch {
 
 // The interpreter loop of both kernels for thread `tid` (row tid mod n).  Every form of one operation ends in the same field
 // operation (the goto targets after the switch), so a fused form costs its operand fetches and no second copy of the arithmetic.
+// The sums of two products (FOLD and the merged HORNER forms) share one tail.
 template <int NREGS, int THREADS, bool SMEM, class Launch>
 __device__ __forceinline__ void run_program(const Launch &L, uint32_t tid) {
     constexpr bool FLAG = std::is_same<Launch, FlagLaunch>::value;
@@ -73,7 +74,7 @@ __device__ __forceinline__ void run_program(const Launch &L, uint32_t tid) {
     auto arg = [&]() { return L.code[++pc].imm; };   // the OP_ARG word after the current instruction
     for (; pc < L.ncode; ++pc) {
         const Instr in = L.code[pc];
-        Fr x, y;
+        Fr x, y, z, w;
         switch (in.op) {
         case OP_LOADCOL: regs.set(in.dst, col(in.imm)); continue;
         case OP_LOADCONST: regs.set(in.dst, cst(in.imm)); continue;
@@ -116,11 +117,17 @@ __device__ __forceinline__ void run_program(const Launch &L, uint32_t tid) {
             if constexpr (!FLAG) acc2 = fp_add(fp_mul(acc2, cst(in.imm)), in.op == OP_HORNER2 ? regs.get(in.a) : col(arg()));
             continue;
         case OP_FOLD: case OP_FOLD_C:
-            if constexpr (!FLAG) {
-                acc = fp_add(fp_mul(acc, cst(in.imm)), fp_mul(in.op == OP_FOLD ? regs.get(in.a) : col(arg()), acc2));
-                acc2 = Fr::zero();
-            }
-            continue;
+            if constexpr (FLAG) continue;
+            else { x = acc; y = cst(in.imm); z = in.op == OP_FOLD ? regs.get(in.a) : col(arg()); w = acc2; goto mac; }
+        case OP_HORNER_M: case OP_HORNER2_M:
+            if constexpr (FLAG) continue;
+            else if constexpr (!SMEM) {
+                // the local-memory build (programs of > 16 registers) keeps its register budget: product first, then the root
+                const Fr t = fp_mul(regs.get(in.a), regs.get(in.b));
+                if (in.op == OP_HORNER_M) acc = fp_add(fp_mul(acc, cst(in.imm)), t);
+                else acc2 = fp_add(fp_mul(acc2, cst(in.imm)), t);
+                continue;
+            } else { x = in.op == OP_HORNER_M ? acc : acc2; y = cst(in.imm); z = regs.get(in.a); w = regs.get(in.b); goto mac; }
         case OP_STORE:
             if constexpr (!FLAG) fp_store(L.outs[in.imm] + (size_t)row * L.out_stride + L.out_offset, regs.get(in.a));
             continue;
@@ -132,7 +139,15 @@ __device__ __forceinline__ void run_program(const Launch &L, uint32_t tid) {
         }
     add: regs.set(in.dst, fp_add(x, y)); continue;
     sub: regs.set(in.dst, fp_sub(x, y)); continue;
-    mul: regs.set(in.dst, fp_mul(x, y));
+    mul: regs.set(in.dst, fp_mul(x, y)); continue;
+    mac: {   // x * y + z * w, one reduction: FOLD and the merged HORNER forms
+        const Fr r = fp_mul_add_mul(x, y, z, w);
+        if (in.op == OP_HORNER2_M) acc2 = r;
+        else {
+            acc = r;
+            if (in.op != OP_HORNER_M) acc2 = Fr::zero();   // FOLD
+        }
+    }
     }
 }
 

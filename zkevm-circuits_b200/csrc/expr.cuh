@@ -45,6 +45,10 @@ enum : uint8_t {
     OP_HORNER_C = 40,   // OP_HORNER / OP_HORNER2 / OP_FOLD with the term a column: consts[imm] as before, the column in OP_ARG
     OP_HORNER2_C = 41,
     OP_FOLD_C = 42,
+    // Merged products (ProgramBuilder::merge_products): a register-register OP_MUL whose result is read once, by a HORNER / HORNER2
+    // root, is evaluated inside the root as a sum of two products with one Montgomery reduction (fp_mul_add_mul).
+    OP_HORNER_M = 43,   // acc = acc * consts[imm] + reg[a] * reg[b]
+    OP_HORNER2_M = 44,  // acc2 = acc2 * consts[imm] + reg[a] * reg[b]
 };
 
 struct alignas(8) Instr {
@@ -141,6 +145,7 @@ public:
 private:
     ExprBuilder &eb;
     void fuse(size_t begin);
+    static void merge_products(std::vector<Instr> &code);
 };
 
 // Peephole pass over the code of one scope, code[begin..): an OP_LOADCOL / OP_LOADCONST whose register is read exactly once
@@ -202,8 +207,64 @@ inline void ProgramBuilder::fuse(size_t begin) {
         out.push_back(Instr{(uint8_t)(base + form), in.dst, (uint8_t)(form < FORM_CC ? reg : 0), 0, code[s[first]].imm});
         if (form >= FORM_CC) out.push_back(Instr{OP_ARG, 0, 0, 0, code[s[1]].imm});
     }
+    merge_products(out);
     code.resize(begin);
     code.insert(code.end(), out.begin(), out.end());
+}
+
+// Second peephole step, on the operand-fused code of one scope: a register-register OP_MUL whose register is read exactly once
+// before it is written again, by a HORNER / HORNER2 root, and whose operand registers are not written before that read, moves
+// into the root (OP_HORNER_M / OP_HORNER2_M): acc * y + a * b then costs one Montgomery reduction instead of two.  A product read
+// twice, or read by anything else, stays an OP_MUL.  Operand order is kept and the result is the same canonical element;
+// registers are only dropped, as in fuse.  (Sums of two products in ADD / SUB are not merged: their tail would keep four
+// operands and both accumulators live and push the interpreter past its register budget.)
+inline void ProgramBuilder::merge_products(std::vector<Instr> &code) {
+    const size_t n = code.size();
+    auto reg_reads = [](const Instr &in, int s) {   // does operand slot s (0: a, 1: b) of `in` read a register
+        const uint8_t op = in.op;
+        if (op == OP_ADD || op == OP_SUB || op == OP_MUL) return true;
+        if (s != 0) return false;
+        if (op == OP_NEG || op == OP_HORNER || op == OP_HORNER2 || op == OP_FOLD || op == OP_STORE || op == OP_FLAG) return true;
+        return op >= OP_ADD_RC && op < OP_MUL_RC + 8 && (op & 7) < FORM_CC;
+    };
+    auto reg_writes = [](const Instr &in) {
+        const uint8_t op = in.op;
+        return op == OP_LOADCOL || op == OP_LOADCONST || op == OP_ADD || op == OP_SUB || op == OP_MUL || op == OP_NEG ||
+               (op >= OP_ADD_RC && op < OP_MUL_RC + 8);
+    };
+    std::vector<int64_t> reader(n, -1);   // for a mergeable OP_MUL: the index of its one reader
+    for (size_t i = 0; i < n; ++i) {
+        const Instr &m = code[i];
+        if (m.op != OP_MUL) continue;
+        int uses = 0;
+        size_t user = 0;
+        for (size_t j = i + 1; j < n && uses < 2; ++j) {
+            for (int s = 0; s < 2; ++s)
+                if (reg_reads(code[j], s) && (s == 0 ? code[j].a : code[j].b) == m.dst) { ++uses; user = j; }
+            if (reg_writes(code[j]) && code[j].dst == m.dst) break;
+        }
+        if (uses != 1) continue;
+        bool intact = true;
+        for (size_t j = i + 1; j < user; ++j)
+            if (reg_writes(code[j]) && (code[j].dst == m.a || code[j].dst == m.b)) intact = false;
+        if (intact) reader[i] = (int64_t)user;
+    }
+    std::vector<int64_t> prod(n, -1);   // the mergeable product read by each root
+    for (size_t i = 0; i < n; ++i)
+        if (reader[i] >= 0 && (code[reader[i]].op == OP_HORNER || code[reader[i]].op == OP_HORNER2)) prod[reader[i]] = (int64_t)i;
+    std::vector<bool> merged(n, false);
+    std::vector<Instr> out;
+    for (size_t j = 0; j < n; ++j) {
+        Instr in = code[j];
+        if (prod[j] >= 0) {
+            in = Instr{(uint8_t)(in.op == OP_HORNER ? OP_HORNER_M : OP_HORNER2_M), 0, code[prod[j]].a, code[prod[j]].b, in.imm};
+            merged[prod[j]] = true;
+        }
+        out.push_back(in);
+    }
+    code.clear();
+    for (size_t j = 0; j < n; ++j)
+        if (!merged[j]) code.push_back(out[j]);
 }
 
 inline bool ProgramBuilder::scope(const std::vector<Root> &roots) {

@@ -346,9 +346,322 @@ FF_HD Fp<PR> fp_mul(const Fp<PR> &a, const Fp<PR> &b) { return fp_mul_t<PR, true
 template <class PR>
 FF_HD Fp<PR> fp_mul_lazy(const Fp<PR> &a, const Fp<PR> &b) { return fp_mul_t<PR, false>(a, b); }
 
+// ---------------------------------------------------------------------------------------------------------
+// Squaring: the 512-bit square T (16 limbs), then one REDC.  A square needs 36 limb products instead of 64 (28 cross products,
+// doubled, plus 8 diagonal ones).  REDC(T) = (T + M p) / R < T / R + p, so every T < R p gives a value < 2p and one conditional
+// subtraction makes it canonical: the same field element, bit for bit, as the word-serial fp_mul(a, a).
+// ---------------------------------------------------------------------------------------------------------
+#if defined(__CUDA_ARCH__)
+namespace detail {
+// c[0 .. 2K) += (e[0], .., e[K-1]) * b, e[j] * b as the lo/hi pair on limbs 2j, 2j+1 -- one carry chain; the carry out is added to
+// c[2K], which the callers keep free of product limbs (it only ever holds earlier carries, so it cannot overflow)
+template <int K>
+FF_D void mad_row(uint32_t *c, const uint32_t *e, uint32_t b) {
+    if constexpr (K == 4) {
+        chain_mad(c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7], c[8], e[0], e[1], e[2], e[3], b);
+    } else if constexpr (K == 3) {
+        asm("mad.lo.cc.u32 %0, %7, %10, %0;\n\t"
+            "madc.hi.cc.u32 %1, %7, %10, %1;\n\t"
+            "madc.lo.cc.u32 %2, %8, %10, %2;\n\t"
+            "madc.hi.cc.u32 %3, %8, %10, %3;\n\t"
+            "madc.lo.cc.u32 %4, %9, %10, %4;\n\t"
+            "madc.hi.cc.u32 %5, %9, %10, %5;\n\t"
+            "addc.u32 %6, %6, 0;"
+            : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3]), "+r"(c[4]), "+r"(c[5]), "+r"(c[6])
+            : "r"(e[0]), "r"(e[1]), "r"(e[2]), "r"(b));
+    } else if constexpr (K == 2) {
+        asm("mad.lo.cc.u32 %0, %5, %7, %0;\n\t"
+            "madc.hi.cc.u32 %1, %5, %7, %1;\n\t"
+            "madc.lo.cc.u32 %2, %6, %7, %2;\n\t"
+            "madc.hi.cc.u32 %3, %6, %7, %3;\n\t"
+            "addc.u32 %4, %4, 0;"
+            : "+r"(c[0]), "+r"(c[1]), "+r"(c[2]), "+r"(c[3]), "+r"(c[4])
+            : "r"(e[0]), "r"(e[1]), "r"(b));
+    } else {
+        static_assert(K == 1, "rows of 1 to 4 products");
+        asm("mad.lo.cc.u32 %0, %3, %4, %0;\n\t"
+            "madc.hi.cc.u32 %1, %3, %4, %1;\n\t"
+            "addc.u32 %2, %2, 0;"
+            : "+r"(c[0]), "+r"(c[1]), "+r"(c[2])
+            : "r"(e[0]), "r"(b));
+    }
+}
+
+// Column-aligned accumulators of a 512-bit value: E collects the rows that start on an even column, O those that start on an odd
+// one (both indexed by absolute column).
+struct Wide {
+    uint32_t E[17], O[17];
+    FF_D Wide() {
+#pragma unroll
+        for (int i = 0; i < 17; ++i) E[i] = O[i] = 0;
+    }
+    // T = E + O (< 2^512)
+    FF_D void sum(uint32_t T[16]) const {
+        T[0] = E[0];
+        asm("add.cc.u32 %0, %15, %30;\n\t"
+            "addc.cc.u32 %1, %16, %31;\n\t"
+            "addc.cc.u32 %2, %17, %32;\n\t"
+            "addc.cc.u32 %3, %18, %33;\n\t"
+            "addc.cc.u32 %4, %19, %34;\n\t"
+            "addc.cc.u32 %5, %20, %35;\n\t"
+            "addc.cc.u32 %6, %21, %36;\n\t"
+            "addc.cc.u32 %7, %22, %37;\n\t"
+            "addc.cc.u32 %8, %23, %38;\n\t"
+            "addc.cc.u32 %9, %24, %39;\n\t"
+            "addc.cc.u32 %10, %25, %40;\n\t"
+            "addc.cc.u32 %11, %26, %41;\n\t"
+            "addc.cc.u32 %12, %27, %42;\n\t"
+            "addc.cc.u32 %13, %28, %43;\n\t"
+            "addc.u32 %14, %29, %44;"
+            : "=r"(T[1]), "=r"(T[2]), "=r"(T[3]), "=r"(T[4]), "=r"(T[5]), "=r"(T[6]), "=r"(T[7]), "=r"(T[8]), "=r"(T[9]), "=r"(T[10]),
+              "=r"(T[11]), "=r"(T[12]), "=r"(T[13]), "=r"(T[14]), "=r"(T[15])
+            : "r"(E[1]), "r"(E[2]), "r"(E[3]), "r"(E[4]), "r"(E[5]), "r"(E[6]), "r"(E[7]), "r"(E[8]), "r"(E[9]), "r"(E[10]), "r"(E[11]),
+              "r"(E[12]), "r"(E[13]), "r"(E[14]), "r"(E[15]),
+              "r"(O[1]), "r"(O[2]), "r"(O[3]), "r"(O[4]), "r"(O[5]), "r"(O[6]), "r"(O[7]), "r"(O[8]), "r"(O[9]), "r"(O[10]), "r"(O[11]),
+              "r"(O[12]), "r"(O[13]), "r"(O[14]), "r"(O[15]));
+    }
+};
+
+// T = a^2: the 28 cross products a_i a_j (i < j) in rows of one multiplier -- a_i * (a_{i+1}, a_{i+3}, ..) starts on odd column
+// 2i + 1 (into O), a_i * (a_{i+2}, a_{i+4}, ..) on even column 2i + 2 (into E) -- then doubled, plus the diagonal a_i^2 at 2i, 2i + 1
+FF_D void wide_sqr(const uint32_t *a, uint32_t T[16]) {
+    Wide w;
+#pragma unroll
+    for (int i = 0; i < 7; ++i) {
+        uint32_t od[4], ev[4];
+        int no = 0, ne = 0;
+#pragma unroll
+        for (int j = i + 1; j < 8; j += 2) od[no++] = a[j];
+#pragma unroll
+        for (int j = i + 2; j < 8; j += 2) ev[ne++] = a[j];
+        switch (no) {
+        case 4: mad_row<4>(w.O + 2 * i + 1, od, a[i]); break;
+        case 3: mad_row<3>(w.O + 2 * i + 1, od, a[i]); break;
+        case 2: mad_row<2>(w.O + 2 * i + 1, od, a[i]); break;
+        default: mad_row<1>(w.O + 2 * i + 1, od, a[i]); break;
+        }
+        switch (ne) {
+        case 3: mad_row<3>(w.E + 2 * i + 2, ev, a[i]); break;
+        case 2: mad_row<2>(w.E + 2 * i + 2, ev, a[i]); break;
+        case 1: mad_row<1>(w.E + 2 * i + 2, ev, a[i]); break;
+        default: break;
+        }
+    }
+    w.sum(T);
+    // T = 2T + sum a_i^2 2^(64 i)  (< 2^512: it is a^2)
+    asm("add.cc.u32 %0, %0, %0;\n\t"
+        "addc.cc.u32 %1, %1, %1;\n\t"
+        "addc.cc.u32 %2, %2, %2;\n\t"
+        "addc.cc.u32 %3, %3, %3;\n\t"
+        "addc.cc.u32 %4, %4, %4;\n\t"
+        "addc.cc.u32 %5, %5, %5;\n\t"
+        "addc.cc.u32 %6, %6, %6;\n\t"
+        "addc.cc.u32 %7, %7, %7;\n\t"
+        "addc.cc.u32 %8, %8, %8;\n\t"
+        "addc.cc.u32 %9, %9, %9;\n\t"
+        "addc.cc.u32 %10, %10, %10;\n\t"
+        "addc.cc.u32 %11, %11, %11;\n\t"
+        "addc.cc.u32 %12, %12, %12;\n\t"
+        "addc.cc.u32 %13, %13, %13;\n\t"
+        "addc.cc.u32 %14, %14, %14;\n\t"
+        "addc.u32 %15, %15, %15;\n\t"
+        "mad.lo.cc.u32 %0, %16, %16, %0;\n\t"
+        "madc.hi.cc.u32 %1, %16, %16, %1;\n\t"
+        "madc.lo.cc.u32 %2, %17, %17, %2;\n\t"
+        "madc.hi.cc.u32 %3, %17, %17, %3;\n\t"
+        "madc.lo.cc.u32 %4, %18, %18, %4;\n\t"
+        "madc.hi.cc.u32 %5, %18, %18, %5;\n\t"
+        "madc.lo.cc.u32 %6, %19, %19, %6;\n\t"
+        "madc.hi.cc.u32 %7, %19, %19, %7;\n\t"
+        "madc.lo.cc.u32 %8, %20, %20, %8;\n\t"
+        "madc.hi.cc.u32 %9, %20, %20, %9;\n\t"
+        "madc.lo.cc.u32 %10, %21, %21, %10;\n\t"
+        "madc.hi.cc.u32 %11, %21, %21, %11;\n\t"
+        "madc.lo.cc.u32 %12, %22, %22, %12;\n\t"
+        "madc.hi.cc.u32 %13, %22, %22, %13;\n\t"
+        "madc.lo.cc.u32 %14, %23, %23, %14;\n\t"
+        "madc.hi.u32 %15, %23, %23, %15;"
+        : "+r"(T[0]), "+r"(T[1]), "+r"(T[2]), "+r"(T[3]), "+r"(T[4]), "+r"(T[5]), "+r"(T[6]), "+r"(T[7]), "+r"(T[8]), "+r"(T[9]),
+          "+r"(T[10]), "+r"(T[11]), "+r"(T[12]), "+r"(T[13]), "+r"(T[14]), "+r"(T[15])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(a[4]), "r"(a[5]), "r"(a[6]), "r"(a[7]));
+}
+
+// REDC: T (16 limbs, T < R p)  ->  T / R mod p, canonical.  The low half is reduced word by word in the running-total frame of
+// fp_mul_t (X at column 0, 9 limbs; Y at column 1, 8 limbs): round i zeroes column 0 with m = x0 * INV and shifts by one limb; the
+// shifted-out stray limb joins column 0 of the next frame, its carry entering the m * p_odd chain.  (T_lo + M p) / R <= p, and the
+// high half is added at the end: < T / R + p < 2p.
+template <class PR>
+FF_D Fp<PR> redc(const uint32_t T[16]) {
+    constexpr uint32_t p0 = PR::P(0), p1 = PR::P(1), p2 = PR::P(2), p3 = PR::P(3), p4 = PR::P(4), p5 = PR::P(5), p6 = PR::P(6), p7 = PR::P(7);
+    uint32_t x0 = T[0], x1 = T[1], x2 = T[2], x3 = T[3], x4 = T[4], x5 = T[5], x6 = T[6], x7 = T[7], x8 = 0;
+    uint32_t y0 = 0, y1 = 0, y2 = 0, y3 = 0, y4 = 0, y5 = 0, y6 = 0, y7 = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        uint32_t m;
+        if (i == 0) {
+            m = x0 * PR::INV;
+            chain_mad_nc(y0, y1, y2, y3, y4, y5, y6, y7, p1, p3, p5, p7, m);
+        } else {
+            // divide the total by 2^32 : X' = Y,  Y' = X >> 64,  stray limb x1 joins column 0
+            const uint32_t s = x1;
+            const uint32_t t0 = x2, t1 = x3, t2 = x4, t3 = x5, t4 = x6, t5 = x7, t6 = x8;
+            x0 = y0; x1 = y1; x2 = y2; x3 = y3; x4 = y4; x5 = y5; x6 = y6; x7 = y7; x8 = 0;
+            y0 = t0; y1 = t1; y2 = t2; y3 = t3; y4 = t4; y5 = t5; y6 = t6; y7 = 0;
+            // Y' < 2^224 plus the carry plus m * (p1 + p3 2^64 + ..) < 2^254: the chain cannot overflow
+            asm("add.cc.u32 %0, %0, %10;\n\t"
+                "mul.lo.u32 %9, %0, %11;\n\t"
+                "madc.lo.cc.u32 %1, %12, %9, %1;\n\t"
+                "madc.hi.cc.u32 %2, %12, %9, %2;\n\t"
+                "madc.lo.cc.u32 %3, %13, %9, %3;\n\t"
+                "madc.hi.cc.u32 %4, %13, %9, %4;\n\t"
+                "madc.lo.cc.u32 %5, %14, %9, %5;\n\t"
+                "madc.hi.cc.u32 %6, %14, %9, %6;\n\t"
+                "madc.lo.cc.u32 %7, %15, %9, %7;\n\t"
+                "madc.hi.u32 %8, %15, %9, %8;"
+                : "+r"(x0), "+r"(y0), "+r"(y1), "+r"(y2), "+r"(y3), "+r"(y4), "+r"(y5), "+r"(y6), "+r"(y7), "=r"(m)
+                : "r"(s), "r"(PR::INV), "r"(p1), "r"(p3), "r"(p5), "r"(p7));
+        }
+        chain_mad(x0, x1, x2, x3, x4, x5, x6, x7, x8, p0, p2, p4, p6, m);
+    }
+    // result = (X >> 32) + Y + T_hi  (< 2p), then one conditional subtraction
+    Fp<PR> r;
+    asm("add.cc.u32 %0, %8, %16;\n\t"
+        "addc.cc.u32 %1, %9, %17;\n\t"
+        "addc.cc.u32 %2, %10, %18;\n\t"
+        "addc.cc.u32 %3, %11, %19;\n\t"
+        "addc.cc.u32 %4, %12, %20;\n\t"
+        "addc.cc.u32 %5, %13, %21;\n\t"
+        "addc.cc.u32 %6, %14, %22;\n\t"
+        "addc.u32 %7, %15, %23;"
+        : "=r"(r.l[0]), "=r"(r.l[1]), "=r"(r.l[2]), "=r"(r.l[3]), "=r"(r.l[4]), "=r"(r.l[5]), "=r"(r.l[6]), "=r"(r.l[7])
+        : "r"(x1), "r"(x2), "r"(x3), "r"(x4), "r"(x5), "r"(x6), "r"(x7), "r"(x8),
+          "r"(y0), "r"(y1), "r"(y2), "r"(y3), "r"(y4), "r"(y5), "r"(y6), "r"(y7));
+    asm("add.cc.u32 %0, %0, %8;\n\t"
+        "addc.cc.u32 %1, %1, %9;\n\t"
+        "addc.cc.u32 %2, %2, %10;\n\t"
+        "addc.cc.u32 %3, %3, %11;\n\t"
+        "addc.cc.u32 %4, %4, %12;\n\t"
+        "addc.cc.u32 %5, %5, %13;\n\t"
+        "addc.cc.u32 %6, %6, %14;\n\t"
+        "addc.u32 %7, %7, %15;"
+        : "+r"(r.l[0]), "+r"(r.l[1]), "+r"(r.l[2]), "+r"(r.l[3]), "+r"(r.l[4]), "+r"(r.l[5]), "+r"(r.l[6]), "+r"(r.l[7])
+        : "r"(T[8]), "r"(T[9]), "r"(T[10]), "r"(T[11]), "r"(T[12]), "r"(T[13]), "r"(T[14]), "r"(T[15]));
+    Fp<PR> t;
+    uint32_t borrow;
+    asm("sub.cc.u32 %0, %9, %17;\n\t"
+        "subc.cc.u32 %1, %10, %18;\n\t"
+        "subc.cc.u32 %2, %11, %19;\n\t"
+        "subc.cc.u32 %3, %12, %20;\n\t"
+        "subc.cc.u32 %4, %13, %21;\n\t"
+        "subc.cc.u32 %5, %14, %22;\n\t"
+        "subc.cc.u32 %6, %15, %23;\n\t"
+        "subc.cc.u32 %7, %16, %24;\n\t"
+        "subc.u32 %8, 0, 0;"
+        : "=r"(t.l[0]), "=r"(t.l[1]), "=r"(t.l[2]), "=r"(t.l[3]), "=r"(t.l[4]), "=r"(t.l[5]), "=r"(t.l[6]), "=r"(t.l[7]), "=r"(borrow)
+        : "r"(r.l[0]), "r"(r.l[1]), "r"(r.l[2]), "r"(r.l[3]), "r"(r.l[4]), "r"(r.l[5]), "r"(r.l[6]), "r"(r.l[7]),
+          "r"(p0), "r"(p1), "r"(p2), "r"(p3), "r"(p4), "r"(p5), "r"(p6), "r"(p7));
+#pragma unroll
+    for (int i = 0; i < 8; ++i) r.l[i] = borrow ? r.l[i] : t.l[i];
+    return r;
+}
+}  // namespace detail
+#endif
+
 template <class PR>
 FF_HD Fp<PR> fp_sqr(const Fp<PR> &a) {
+#if defined(__CUDA_ARCH__)
+    uint32_t T[16];
+    detail::wide_sqr(a.l, T);
+    return detail::redc<PR>(T);
+#else
     return fp_mul(a, a);
+#endif
+}
+
+// a * b + c * d with one reduction (a, c <= p; b, d < p, so T = a b + c d < 2p^2 < R p).  Word-serial like fp_mul_t, with both
+// products' rows added before each round's m: the same 64 + 64 + 72 products as a wide sum followed by REDC, but only the 17-limb
+// running total is live instead of 34 accumulator limbs.  Bounds: Y' = X >> 64 < 2^224 plus three chains of 4 limbs times one
+// word, each < 2^254 (the top limb of p and of every operand is < 2^30): < 2^256; X' < 2^256 plus three chains < 2^256 each
+// fits 9 limbs.  The result (T + M p) / R < 2p, then one conditional subtraction.
+template <class PR>
+FF_HD Fp<PR> fp_mul_add_mul(const Fp<PR> &a, const Fp<PR> &b, const Fp<PR> &c, const Fp<PR> &d) {
+#if defined(__CUDA_ARCH__)
+    using namespace detail;
+    uint32_t x0 = 0, x1 = 0, x2 = 0, x3 = 0, x4 = 0, x5 = 0, x6 = 0, x7 = 0, x8 = 0;
+    uint32_t y0 = 0, y1 = 0, y2 = 0, y3 = 0, y4 = 0, y5 = 0, y6 = 0, y7 = 0;
+    constexpr uint32_t p0 = PR::P(0), p1 = PR::P(1), p2 = PR::P(2), p3 = PR::P(3), p4 = PR::P(4), p5 = PR::P(5), p6 = PR::P(6), p7 = PR::P(7);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        const uint32_t bi = b.l[i], di = d.l[i];
+        if (i == 0) {
+            chain_mad_nc(y0, y1, y2, y3, y4, y5, y6, y7, a.l[1], a.l[3], a.l[5], a.l[7], bi);
+        } else {
+            uint32_t s = x1;
+            uint32_t t0 = x2, t1 = x3, t2 = x4, t3 = x5, t4 = x6, t5 = x7, t6 = x8;
+            x0 = y0; x1 = y1; x2 = y2; x3 = y3; x4 = y4; x5 = y5; x6 = y6; x7 = y7; x8 = 0;
+            y0 = t0; y1 = t1; y2 = t2; y3 = t3; y4 = t4; y5 = t5; y6 = t6; y7 = 0;
+            chain_stray_mad_nc(x0, s, y0, y1, y2, y3, y4, y5, y6, y7, a.l[1], a.l[3], a.l[5], a.l[7], bi);
+        }
+        chain_mad_nc(y0, y1, y2, y3, y4, y5, y6, y7, c.l[1], c.l[3], c.l[5], c.l[7], di);
+        chain_mad(x0, x1, x2, x3, x4, x5, x6, x7, x8, a.l[0], a.l[2], a.l[4], a.l[6], bi);
+        chain_mad(x0, x1, x2, x3, x4, x5, x6, x7, x8, c.l[0], c.l[2], c.l[4], c.l[6], di);
+        const uint32_t m = x0 * PR::INV;
+        chain_mad(x0, x1, x2, x3, x4, x5, x6, x7, x8, p0, p2, p4, p6, m);
+        chain_mad_nc(y0, y1, y2, y3, y4, y5, y6, y7, p1, p3, p5, p7, m);
+    }
+    Fp<PR> r, t;
+    asm("add.cc.u32 %0, %8, %16;\n\t"
+        "addc.cc.u32 %1, %9, %17;\n\t"
+        "addc.cc.u32 %2, %10, %18;\n\t"
+        "addc.cc.u32 %3, %11, %19;\n\t"
+        "addc.cc.u32 %4, %12, %20;\n\t"
+        "addc.cc.u32 %5, %13, %21;\n\t"
+        "addc.cc.u32 %6, %14, %22;\n\t"
+        "addc.u32 %7, %15, %23;"
+        : "=r"(r.l[0]), "=r"(r.l[1]), "=r"(r.l[2]), "=r"(r.l[3]), "=r"(r.l[4]), "=r"(r.l[5]), "=r"(r.l[6]), "=r"(r.l[7])
+        : "r"(x1), "r"(x2), "r"(x3), "r"(x4), "r"(x5), "r"(x6), "r"(x7), "r"(x8),
+          "r"(y0), "r"(y1), "r"(y2), "r"(y3), "r"(y4), "r"(y5), "r"(y6), "r"(y7));
+    uint32_t borrow;
+    asm("sub.cc.u32 %0, %9, %17;\n\t"
+        "subc.cc.u32 %1, %10, %18;\n\t"
+        "subc.cc.u32 %2, %11, %19;\n\t"
+        "subc.cc.u32 %3, %12, %20;\n\t"
+        "subc.cc.u32 %4, %13, %21;\n\t"
+        "subc.cc.u32 %5, %14, %22;\n\t"
+        "subc.cc.u32 %6, %15, %23;\n\t"
+        "subc.cc.u32 %7, %16, %24;\n\t"
+        "subc.u32 %8, 0, 0;"
+        : "=r"(t.l[0]), "=r"(t.l[1]), "=r"(t.l[2]), "=r"(t.l[3]), "=r"(t.l[4]), "=r"(t.l[5]), "=r"(t.l[6]), "=r"(t.l[7]), "=r"(borrow)
+        : "r"(r.l[0]), "r"(r.l[1]), "r"(r.l[2]), "r"(r.l[3]), "r"(r.l[4]), "r"(r.l[5]), "r"(r.l[6]), "r"(r.l[7]),
+          "r"(p0), "r"(p1), "r"(p2), "r"(p3), "r"(p4), "r"(p5), "r"(p6), "r"(p7));
+#pragma unroll
+    for (int i = 0; i < 8; ++i) r.l[i] = borrow ? r.l[i] : t.l[i];
+    return r;
+#else
+    return fp_add(fp_mul(a, b), fp_mul(c, d));
+#endif
+}
+
+// a * b - c * d with one reduction, as a * b + (p - c) * d: p - c is in (0, p], so T < 2p^2 as for the sum
+template <class PR>
+FF_HD Fp<PR> fp_mul_sub_mul(const Fp<PR> &a, const Fp<PR> &b, const Fp<PR> &c, const Fp<PR> &d) {
+#if defined(__CUDA_ARCH__)
+    Fp<PR> nc;
+    asm("sub.cc.u32 %0, %8, %16;\n\t"
+        "subc.cc.u32 %1, %9, %17;\n\t"
+        "subc.cc.u32 %2, %10, %18;\n\t"
+        "subc.cc.u32 %3, %11, %19;\n\t"
+        "subc.cc.u32 %4, %12, %20;\n\t"
+        "subc.cc.u32 %5, %13, %21;\n\t"
+        "subc.cc.u32 %6, %14, %22;\n\t"
+        "subc.u32 %7, %15, %23;"
+        : "=r"(nc.l[0]), "=r"(nc.l[1]), "=r"(nc.l[2]), "=r"(nc.l[3]), "=r"(nc.l[4]), "=r"(nc.l[5]), "=r"(nc.l[6]), "=r"(nc.l[7])
+        : "r"(PR::P(0)), "r"(PR::P(1)), "r"(PR::P(2)), "r"(PR::P(3)), "r"(PR::P(4)), "r"(PR::P(5)), "r"(PR::P(6)), "r"(PR::P(7)),
+          "r"(c.l[0]), "r"(c.l[1]), "r"(c.l[2]), "r"(c.l[3]), "r"(c.l[4]), "r"(c.l[5]), "r"(c.l[6]), "r"(c.l[7]));
+    return fp_mul_add_mul(a, b, nc, d);
+#else
+    return fp_sub(fp_mul(a, b), fp_mul(c, d));
+#endif
 }
 
 #if defined(__CUDACC__)

@@ -5,6 +5,8 @@
 // ("XYZZ": x = X/ZZ, y = Y/ZZZ, ZZ^3 = ZZZ^2) coordinates: a mixed addition is 8M + 2S with no inversion and a
 // cheap identity test (ZZ == 0).  Formulas: EFD "madd-2008-s", "add-2008-s", "dbl-2008-s-1", "mdbl-2008-s-1"
 // for short Weierstrass curves with a = 0.
+// On the device the squarings use fp_sqr's dedicated square and each y3 = A*B - C*D one reduction (fp_mul_sub_mul); both
+// return the same canonical elements as separate multiplies, so the points are bit-identical.
 #pragma once
 #include "ff.cuh"
 
@@ -42,7 +44,7 @@ FF_HD G1Xyzz g1_dbl_affine(const G1Affine &p) {
     Fq xx = fp_sqr(p.x);
     Fq m = fp_add(fp_dbl(xx), xx);
     r.x = fp_sub(fp_sqr(m), fp_dbl(s));
-    r.y = fp_sub(fp_mul(m, fp_sub(s, r.x)), fp_mul(w, p.y));
+    r.y = fp_mul_sub_mul(m, fp_sub(s, r.x), w, p.y);
     r.zz = v;
     r.zzz = w;
     return r;
@@ -58,7 +60,7 @@ FF_HD G1Xyzz g1_dbl(const G1Xyzz &p) {
     Fq xx = fp_sqr(p.x);
     Fq m = fp_add(fp_dbl(xx), xx);
     r.x = fp_sub(fp_sqr(m), fp_dbl(s));
-    r.y = fp_sub(fp_mul(m, fp_sub(s, r.x)), fp_mul(w, p.y));
+    r.y = fp_mul_sub_mul(m, fp_sub(s, r.x), w, p.y);
     r.zz = fp_mul(v, p.zz);
     r.zzz = fp_mul(w, p.zzz);
     return r;
@@ -81,7 +83,7 @@ FF_HD void g1_add_mixed(G1Xyzz &acc, const G1Affine &q) {
     Fq ppp = fp_mul(p, pp);
     Fq qq = fp_mul(acc.x, pp);
     Fq x3 = fp_sub(fp_sub(fp_sqr(r), ppp), fp_dbl(qq));
-    Fq y3 = fp_sub(fp_mul(r, fp_sub(qq, x3)), fp_mul(acc.y, ppp));
+    Fq y3 = fp_mul_sub_mul(r, fp_sub(qq, x3), acc.y, ppp);
     acc.x = x3;
     acc.y = y3;
     acc.zz = fp_mul(acc.zz, pp);
@@ -107,7 +109,7 @@ FF_HD void g1_add(G1Xyzz &acc, const G1Xyzz &q) {
     Fq ppp = fp_mul(p, pp);
     Fq qq = fp_mul(u1, pp);
     Fq x3 = fp_sub(fp_sub(fp_sqr(r), ppp), fp_dbl(qq));
-    Fq y3 = fp_sub(fp_mul(r, fp_sub(qq, x3)), fp_mul(s1, ppp));
+    Fq y3 = fp_mul_sub_mul(r, fp_sub(qq, x3), s1, ppp);
     acc.x = x3;
     acc.y = y3;
     acc.zz = fp_mul(fp_mul(acc.zz, q.zz), pp);
