@@ -223,8 +223,9 @@ ZKB_API int32_t zkb_msm_g1_sharded_dev(zkb_ctx *ctx, const uint64_t *scalars_sha
 
 /* zkb_comm_*   NCCL communicator of a context for the multi-GPU create_proof (one process per GPU).  Rank 0 creates a
  * 128-byte unique id, the host layer broadcasts it, every rank calls zkb_comm_init.  With a communicator the proving session
- * stays replicated (identical transcript and proof bytes on every rank) while commitment batches (column i -> rank i mod P) and
- * the quotient's coset parts (part j -> rank j mod P) are dealt across the ranks and exchanged by one all-reduce each.        */
+ * stays replicated (identical transcript and proof bytes on every rank) while independent units -- columns, lookup arguments,
+ * permutation sets, the quotient's coset parts -- are cut into P contiguous blocks (rank r computes block r) and each result is
+ * completed by one in-place all-gather.                                                                                      */
 ZKB_API int32_t zkb_comm_unique_id(uint8_t out[128]);
 ZKB_API int32_t zkb_comm_init(zkb_ctx *ctx, const uint8_t unique_id[128], int32_t rank, int32_t nranks);
 ZKB_API int32_t zkb_comm_destroy(zkb_ctx *ctx);

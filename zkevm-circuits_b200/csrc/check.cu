@@ -1,14 +1,31 @@
-// check.cu -- the bitmap side of the witness check (zkb_check_witness_dev, prover.cu): copy-constraint flags, exact failure counts
-// and the ordered extraction of failure records.
+// check.cu -- the witness check (zkb_check_witness_dev): gate flags from the interpreter's flag build, lookup membership flags,
+// copy-constraint flags, exact failure counts and the ordered extraction of failure records.
 //
 // Every item (a gate, a lookup input set, the copy list) owns a bitmap with one bit per row (per copy for the copy list); bit b of
 // word w stands for row 32 w + b.  Every word is written by exactly one warp with __ballot_sync, so the bitmaps, the counts and the
 // records are the same bytes on every run.  Only the counts and the first `cap` records cross PCIe, never a bitmap.
-#include "common.cuh"
+#include "lookup.cuh"
 
 namespace zkb {
 
 constexpr uint32_t CHECK_THREADS = 256;
+
+struct CheckItem {
+    const uint32_t *bits;   // bit b of word w: row (or copy index) 32 w + b fails
+    uint64_t words;
+    uint32_t kind, index, sub;   // the record fields (zkb_check_record); copies take index = copy index, row = left row
+    uint64_t share, offset;      // extraction: records to write and where (filled by check_collect)
+};
+
+// the same probe as the prover's m_count_kernel, but one bit per row (word i / 32 by __ballot_sync, one writer per word) saying
+// "input row i < usable is not in the table"; launched over all words of the bitmap, rows >= usable vote 0
+__global__ void m_member_kernel(const Fr *__restrict__ f, const Fr *__restrict__ t, uint32_t usable, const uint32_t *__restrict__ slots,
+                                uint32_t mask, uint32_t *__restrict__ bits, uint32_t words) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool missing = i < usable && m_probe(f, i, t, slots, mask) == NOT_IN_TABLE;
+    const uint32_t b = __ballot_sync(0xffffffffu, missing);
+    if ((threadIdx.x & 31) == 0 && (i >> 5) < words) bits[i >> 5] = b;
+}
 
 // one thread per copy (lc, lr, rc, rr); columns index the permutation column list.  An entry out of range votes 0 and lowers
 // *first_bad to its index (atomicMin: the first offending entry whatever the schedule).
@@ -80,7 +97,9 @@ __global__ void __launch_bounds__(CHECK_THREADS) bitmap_extract_kernel(const Che
     }
 }
 
-int32_t copy_flags_device(zkb_ctx *ctx, DevPool &pool, const uint32_t *copies, uint64_t n_copies, const Fr *const *d_perm_cols, uint32_t P,
+// bit i of bits[i / 32]: copy i's two cells differ.  Returns in *first_bad the first entry with a column >= P or a row >= n, or
+// UINT64_MAX; synchronises.
+static int32_t copy_flags_device(zkb_ctx *ctx, DevPool &pool, const uint32_t *copies, uint64_t n_copies, const Fr *const *d_perm_cols, uint32_t P,
                           uint32_t n, uint32_t *bits, uint64_t *first_bad, cudaStream_t st) {
     unsigned long long *d_bad = nullptr;
     ZKB_TRY(pool.alloc(8, (void **)&d_bad));
@@ -98,7 +117,9 @@ int32_t copy_flags_device(zkb_ctx *ctx, DevPool &pool, const uint32_t *copies, u
     return ZKB_OK;
 }
 
-int32_t check_collect(zkb_ctx *ctx, DevPool &pool, const std::vector<CheckItem> &items, const uint32_t *copies, uint64_t *counts_out,
+// exact set-bit count of every item to counts_out, then the first `cap` set bits in item order to records_out (*n_records of them);
+// only counts and records leave the device; synchronises
+static int32_t check_collect(zkb_ctx *ctx, DevPool &pool, const std::vector<CheckItem> &items, const uint32_t *copies, uint64_t *counts_out,
                       zkb_check_record *records_out, uint32_t cap, uint32_t *n_records, cudaStream_t st) {
     ProfScope ps_(ctx, PROF_CHECK_EXTRACT, st);
     const size_t ni = items.size();
@@ -142,3 +163,121 @@ int32_t check_collect(zkb_ctx *ctx, DevPool &pool, const std::vector<CheckItem> 
 }
 
 }  // namespace zkb
+using namespace zkb;
+
+// MockProver::run + assert_satisfied on the device (semantics in zkb200.h): one bitmap per gate (the interpreter's flag build, one
+// CSE scope per gate), per lookup input set (compression as the prover's lookup_prepare computes it, the table's hash set,
+// m_member_kernel) and for the copy list, then exact counts and the first `cap` records (check_collect).
+extern "C" int32_t zkb_check_witness_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, const uint64_t *const *columns_dev,
+                                         const uint64_t *challenges, const uint64_t *theta, const uint32_t *copies_dev, uint64_t n_copies,
+                                         uint64_t *counts_out, zkb_check_record *records_out, uint32_t cap, uint32_t *n_records, void *stream) {
+    ZKB_ARG(ctx && csf && columns_dev && counts_out && n_records && (records_out || cap == 0) && (copies_dev || n_copies == 0));
+    ZKB_ARG(n_copies < (1ull << 32));
+    ZKB_CUDA(cudaSetDevice(ctx->device));
+    Csf cs;
+    ZKB_TRY(load_csf(csf, csf_words, cs));
+    if (cs.nch && !challenges) { set_error("zkb_check_witness_dev: the constraint system has %u challenges and none were given", cs.nch); return ZKB_ERR_ARG; }
+    for (size_t l = 0; l < cs.lookups.size(); ++l)
+        if (cs.lookups[l].table.size() > 1 && !theta) {
+            set_error("zkb_check_witness_dev: lookup %zu has width %zu and needs theta", l, cs.lookups[l].table.size());
+            return ZKB_ERR_ARG;
+        }
+    const std::vector<Fr> ch = host_challenges(challenges, cs.nch);
+    Fr th = Fr::zero();
+    if (theta) memcpy(th.l, theta, sizeof(Fr));
+    cudaStream_t st = pick_stream(ctx, stream);
+    const uint32_t n = 1u << cs.k, words = (n + 31) / 32;
+    const uint32_t usable = n > cs.bf + 1 ? n - cs.bf - 1 : 0;
+    const SlotMap sm(cs, 0);   // the caller's columns are its [fixed | advice | instance] prefix
+    const std::vector<Fr *> cols((Fr *const *)columns_dev, (Fr *const *)columns_dev + sm.sigma0);
+    size_t nsets = 0, maxsets = 0;
+    for (auto &lk : cs.lookups) { nsets += lk.inputs.size(); maxsets = std::max(maxsets, lk.inputs.size()); }
+    const uint64_t copy_words = (n_copies + 31) / 32;
+    DevPool pool;
+    pool.ctx = ctx;
+    Fr **d_cols = nullptr;
+    uint32_t *bits = nullptr;
+    ZKB_TRY(upload_table(pool, cols, &d_cols, st));
+    ZKB_TRY(pool.alloc(((cs.gates.size() + nsets) * words + copy_words) * 4, (void **)&bits));
+    uint32_t *lk_bits = bits + cs.gates.size() * words, *copy_bits = lk_bits + nsets * words;
+    std::vector<CheckItem> items;
+
+    if (!cs.gates.empty()) {   // gates: one scope per gate, no selector folding
+        ProfScope ps_(ctx, PROF_CHECK_GATES, st);
+        ExprBuilder eb;
+        ProgramBuilder pb(eb);
+        std::vector<int64_t> memo(cs.nodes.size(), -1);
+        for (size_t g = 0; g < cs.gates.size(); ++g)
+            if (!pb.scope({{translate(cs, cs.gates[g], eb, sm, ch, memo), ProgramBuilder::FLAG, (uint32_t)g}})) {
+                set_error("gate %zu: %s", g, pb.error.c_str());
+                return ZKB_ERR_ARG;
+            }
+        DeviceProgram dp;
+        ZKB_TRY(upload_program(pool, pb, eb, dp, st));
+        ZKB_TRY(expr_flag_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, bits, words, cs.k, st));
+    }
+    for (size_t g = 0; g < cs.gates.size(); ++g) items.push_back({bits + g * words, words, 0, (uint32_t)g, 0, 0, 0});
+
+    if (nsets) {               // lookups, one argument at a time: compressed inputs and table, the table's hash set, membership bits
+        ProfScope ps_(ctx, PROF_CHECK_LOOKUPS, st);
+        std::vector<Fr *> bufs(maxsets + 1);
+        for (auto &b : bufs) ZKB_TRY(pool.fr(n, &b));
+        uint32_t *slots = nullptr, mask = 0;
+        uint32_t *out = lk_bits;
+        for (size_t l = 0; l < cs.lookups.size(); ++l) {
+            const size_t ns = cs.lookups[l].inputs.size();
+            ZKB_TRY(lookup_compress(ctx, cs, l, sm, ch, th, pool, d_cols, std::vector<Fr *>(bufs.begin(), bufs.begin() + ns), bufs[maxsets], st));
+            ZKB_TRY(table_hash_set(ctx, pool, bufs[maxsets], usable, slots, mask, st));
+            for (size_t j = 0; j < ns; ++j, out += words) {
+                m_member_kernel<<<(n + 255) / 256, 256, 0, st>>>(bufs[j], bufs[maxsets], usable, slots, mask, out, words);
+                ctx->launches++;
+                items.push_back({out, words, 1, (uint32_t)l, (uint32_t)j, 0, 0});
+            }
+            ZKB_CUDA(cudaGetLastError());
+        }
+    }
+
+    {                          // copies
+        ProfScope ps_(ctx, PROF_CHECK_COPIES, st);
+        std::vector<Fr *> pc;
+        for (auto &c : cs.perm) pc.push_back(cols[sm.perm(c)]);
+        Fr **d_pc = nullptr;
+        ZKB_TRY(upload_table(pool, pc, &d_pc, st));
+        uint64_t first_bad = 0;
+        ZKB_TRY(copy_flags_device(ctx, pool, copies_dev, n_copies, d_pc, (uint32_t)pc.size(), n, copy_bits, &first_bad, st));
+        if (first_bad != ~0ull) {
+            set_error("zkb_check_witness_dev: copy constraint %llu is out of range (column >= %zu or row >= %u)", (unsigned long long)first_bad,
+                      pc.size(), n);
+            return ZKB_ERR_ARG;
+        }
+    }
+    items.push_back({copy_bits, copy_words, 2, 0, 0, 0, 0});
+
+    ZKB_TRY(check_collect(ctx, pool, items, copies_dev, counts_out, records_out, cap, n_records, st));
+    // poisoned gate failures: an advice query of the gate reads a row >= usable at the failing row
+    std::vector<std::vector<int32_t>> adv_rots(cs.gates.size());
+    std::vector<bool> adv_rots_done(cs.gates.size(), false);
+    for (uint32_t i = 0; i < *n_records && records_out[i].kind == 0; ++i) {
+        zkb_check_record &r = records_out[i];
+        std::vector<int32_t> &rots = adv_rots[r.index];
+        if (!adv_rots_done[r.index]) {
+            std::vector<uint32_t> stack{cs.gates[r.index]};
+            std::vector<bool> seen(cs.nodes.size(), false);
+            while (!stack.empty()) {
+                const uint32_t v = stack.back();
+                stack.pop_back();
+                if (seen[v]) continue;
+                seen[v] = true;
+                const auto &nd = cs.nodes[v];
+                if (nd[0] == N_ADVICE) rots.push_back((int32_t)nd[2]);
+                else if (nd[0] == N_NEG || nd[0] == N_SCALED) stack.push_back(nd[1]);
+                else if (nd[0] == N_ADD || nd[0] == N_MUL) { stack.push_back(nd[1]); stack.push_back(nd[2]); }
+            }
+            adv_rots_done[r.index] = true;
+        }
+        r.sub = 0;
+        for (int32_t rot : rots)
+            if (((r.row + (uint32_t)rot) & (n - 1)) >= usable) { r.sub = 1; break; }
+    }
+    return ZKB_OK;
+}

@@ -210,21 +210,5 @@ struct DevPool {  // owns device allocations of a pk / session; blocks are recyc
     int32_t fr(uint64_t n, Fr **out) { return alloc(n * sizeof(Fr), (void **)out); }
 };
 
-// ---- witness check (check.cu): one failure bitmap per item -- a gate, a lookup input set, or the copy list -- in report order
-struct CheckItem {
-    const uint32_t *bits;   // bit b of word w: row (or copy index) 32 w + b fails
-    uint64_t words;
-    uint32_t kind, index, sub;   // the record fields (zkb_check_record); copies take index = copy index, row = left row
-    uint64_t share, offset;      // extraction: records to write and where (filled by check_collect)
-};
-// bit i of bits[i / 32]: copy i's two cells differ.  Returns in *first_bad the first entry with a column >= P or a row >= n, or
-// UINT64_MAX; synchronises.
-int32_t copy_flags_device(zkb_ctx *ctx, DevPool &pool, const uint32_t *copies, uint64_t n_copies, const Fr *const *d_perm_cols, uint32_t P,
-                          uint32_t n, uint32_t *bits, uint64_t *first_bad, cudaStream_t st);
-// exact set-bit count of every item to counts_out, then the first `cap` set bits in item order to records_out (*n_records of them);
-// only counts and records leave the device; synchronises
-int32_t check_collect(zkb_ctx *ctx, DevPool &pool, const std::vector<CheckItem> &items, const uint32_t *copies, uint64_t *counts_out,
-                      zkb_check_record *records_out, uint32_t cap, uint32_t *n_records, cudaStream_t st);
-
 enum ScratchSlot { SCR_NTT = 0, SCR_MSM_A = 1, SCR_MSM_B = 2, SCR_MSM_C = 3, SCR_HOSTIO_A = 4, SCR_HOSTIO_B = 5, SCR_MISC = 6, SCR_MISC2 = 7, SCR_MSM_TBL = 8, SCR_COMM = 9, SCR_NTT_DESC = 10, SCR_MSM_D = 11, SCR_COMM_FLAG = 12, SCR_SHARD = 13 };
 }  // namespace zkb

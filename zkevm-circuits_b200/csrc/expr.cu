@@ -178,7 +178,6 @@ static int32_t launch_smem(const Launch &L, uint32_t n, cudaStream_t st) {
     return ZKB_OK;
 }
 
-// d_code / d_cols / d_consts / d_outs are device pointers
 int32_t expr_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int nregs, const Fr *const *d_cols, const Fr *d_consts,
                         Fr *const *d_outs, uint32_t log_n, uint32_t out_stride, uint32_t out_offset, cudaStream_t st) {
     ExprLaunch L{d_code, ncode, d_cols, d_consts, d_outs, log_n, out_stride, out_offset};
@@ -198,8 +197,6 @@ int32_t expr_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int n
     return ZKB_OK;
 }
 
-// the flag build over 2^log_n rows: FLAG(g) writes words [g * words, (g + 1) * words) of `bits` (device pointers as above); the
-// register bands are those of expr_run_device
 int32_t expr_flag_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int nregs, const Fr *const *d_cols, const Fr *d_consts,
                              uint32_t *bits, uint32_t words, uint32_t log_n, cudaStream_t st) {
     FlagLaunch L{d_code, ncode, d_cols, d_consts, bits, words, log_n};

@@ -16,7 +16,7 @@
 #include <string>
 #include <tuple>
 #include <vector>
-#include "ff.cuh"
+#include "common.cuh"
 
 namespace zkb {
 
@@ -360,6 +360,53 @@ inline bool ProgramBuilder::scope(const std::vector<Root> &roots) {
     }
     fuse(begin);
     return true;
+}
+
+// ---- running programs (expr.cu) ---------------------------------------------------------------------------------------
+// d_code / d_cols / d_consts / d_outs are device pointers
+int32_t expr_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int nregs, const Fr *const *d_cols, const Fr *d_consts,
+                        Fr *const *d_outs, uint32_t log_n, uint32_t out_stride, uint32_t out_offset, cudaStream_t st);
+// the flag build over 2^log_n rows: FLAG(g) writes words [g * words, (g + 1) * words) of `bits` (device pointers as above); the
+// register bands are those of expr_run_device
+int32_t expr_flag_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int nregs, const Fr *const *d_cols, const Fr *d_consts,
+                             uint32_t *bits, uint32_t words, uint32_t log_n, cudaStream_t st);
+
+// program bundle uploaded to the device
+struct DeviceProgram {
+    Instr *code = nullptr;
+    uint32_t ncode = 0;
+    int nregs = 0;
+    Fr *consts = nullptr;
+};
+inline int32_t upload_program(DevPool &pool, const ProgramBuilder &pb, const ExprBuilder &eb, DeviceProgram &dp, cudaStream_t st) {
+    dp.ncode = (uint32_t)pb.code.size();
+    dp.nregs = pb.max_regs_used;
+    ZKB_TRY(pool.alloc(pb.code.size() * sizeof(Instr) + 8, (void **)&dp.code));
+    ZKB_TRY(pool.alloc(eb.consts.size() * sizeof(Fr) + 32, (void **)&dp.consts));
+    ZKB_CUDA(cudaMemcpyAsync(dp.code, pb.code.data(), pb.code.size() * sizeof(Instr), cudaMemcpyHostToDevice, st));
+    ZKB_CUDA(cudaMemcpyAsync(dp.consts, eb.consts.data(), eb.consts.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
+    ZKB_CUDA(cudaStreamSynchronize(st));  // host vectors may die after return
+    return ZKB_OK;
+}
+template <class T>
+inline int32_t upload_table(DevPool &pool, const std::vector<T *> &host, T ***dev, cudaStream_t st) {
+    ZKB_TRY(pool.alloc(host.size() * sizeof(T *) + 8, (void **)dev));
+    ZKB_CUDA(cudaMemcpyAsync(*dev, host.data(), host.size() * sizeof(T *), cudaMemcpyHostToDevice, st));
+    ZKB_CUDA(cudaStreamSynchronize(st));
+    return ZKB_OK;
+}
+// one program whose root i is STOREd to outs[i], uploaded with its output table and run over the 2^log_n rows of the d_cols table
+inline int32_t run_store_program(zkb_ctx *ctx, uint32_t log_n, DevPool &pool, ExprBuilder &eb, const std::vector<uint32_t> &roots,
+                                 const std::vector<Fr *> &outs, const Fr *const *d_cols, const std::string &what, cudaStream_t st) {
+    ProgramBuilder pb(eb);
+    std::vector<ProgramBuilder::Root> stores;
+    for (size_t i = 0; i < roots.size(); ++i) stores.push_back({roots[i], ProgramBuilder::STORE, (uint32_t)i});
+    if (!pb.scope(stores)) { set_error("%s: %s", what.c_str(), pb.error.c_str()); return ZKB_ERR_ARG; }
+    DeviceProgram dp;
+    ZKB_TRY(upload_program(pool, pb, eb, dp, st));
+    Fr **d_outs = nullptr;
+    ZKB_TRY(upload_table(pool, outs, &d_outs, st));
+    return expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, log_n, 1, 0, st);
 }
 
 }  // namespace zkb

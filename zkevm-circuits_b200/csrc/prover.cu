@@ -18,10 +18,10 @@
 // size n, SURVEY 8e) by one fused interpreter launch per degree group on the part, each group only on the parts its degree
 // needs (QuotientGroups); all scans / inversions / evaluations are parallel kernels.
 #include "common.cuh"
+#include "csf.cuh"
 #include "expr.cuh"
-#include "blake2b.h"
-#include "poseidon.h"
-#include "keccak.h"
+#include "lookup.cuh"
+#include "transcript.cuh"
 #include <algorithm>
 #include <memory>
 #include <string.h>
@@ -29,141 +29,6 @@
 #include <time.h>
 
 namespace zkb {
-
-int32_t expr_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int nregs, const Fr *const *d_cols, const Fr *d_consts,
-                        Fr *const *d_outs, uint32_t log_n, uint32_t out_stride, uint32_t out_offset, cudaStream_t st);
-int32_t expr_flag_run_device(zkb_ctx *ctx, const Instr *d_code, uint32_t ncode, int nregs, const Fr *const *d_cols, const Fr *d_consts,
-                             uint32_t *bits, uint32_t words, uint32_t log_n, cudaStream_t st);
-
-// ---------------------------------------------------------------------------------------------------------- CSF
-enum { N_CONST = 0, N_FIXED = 1, N_ADVICE = 2, N_INSTANCE = 3, N_CHALLENGE = 4, N_NEG = 5, N_ADD = 6, N_MUL = 7, N_SCALED = 8 };
-constexpr uint32_t CSF_MAGIC = 0x3146535au;
-
-struct CsfLookup {
-    std::vector<std::vector<uint32_t>> inputs;
-    std::vector<uint32_t> table;
-};
-struct Csf {
-    uint32_t k = 0, nf = 0, na = 0, ni = 0, nch = 0, bf = 0, d = 0, nphases = 0;
-    std::vector<uint32_t> adv_phase, ch_phase;
-    std::vector<std::array<uint32_t, 3>> nodes;
-    std::vector<Fr> consts;
-    std::vector<uint32_t> gates;
-    std::vector<CsfLookup> lookups;
-    std::vector<std::array<uint32_t, 2>> perm;
-    std::vector<std::array<int32_t, 2>> advq, fixq, instq;
-};
-
-static bool parse_csf(const uint32_t *w, uint64_t nw, Csf &c) {
-    if (nw < 18 || w[0] != CSF_MAGIC) { set_error("CSF: bad magic / too short"); return false; }
-    c.k = w[1]; c.nf = w[2]; c.na = w[3]; c.ni = w[4]; c.nch = w[5]; c.bf = w[6]; c.d = w[7]; c.nphases = w[8];
-    const uint32_t n_nodes = w[9], n_consts = w[10], n_gates = w[11], n_lookups = w[12], n_perm = w[13], n_aq = w[14], n_fq = w[15], n_iq = w[16];
-    uint64_t p = 18;
-    auto need = [&](uint64_t cnt) { return p + cnt <= nw; };
-    if (!need(c.na + c.nch)) { set_error("CSF: truncated"); return false; }
-    c.adv_phase.assign(w + p, w + p + c.na); p += c.na;
-    c.ch_phase.assign(w + p, w + p + c.nch); p += c.nch;
-    if (!need(3ull * n_nodes)) { set_error("CSF: truncated nodes"); return false; }
-    c.nodes.resize(n_nodes);
-    for (uint32_t i = 0; i < n_nodes; ++i) { c.nodes[i] = {w[p], w[p + 1], w[p + 2]}; p += 3; }
-    if (!need(8ull * n_consts)) { set_error("CSF: truncated consts"); return false; }
-    c.consts.resize(n_consts);
-    for (uint32_t i = 0; i < n_consts; ++i) { memcpy(c.consts[i].l, w + p, 32); p += 8; }
-    if (!need(n_gates)) { set_error("CSF: truncated gates"); return false; }
-    c.gates.assign(w + p, w + p + n_gates); p += n_gates;
-    c.lookups.resize(n_lookups);
-    for (uint32_t l = 0; l < n_lookups; ++l) {
-        if (!need(2)) { set_error("CSF: truncated lookups"); return false; }
-        const uint32_t nsets = w[p], width = w[p + 1];
-        p += 2;
-        if (nsets == 0 || width == 0 || nsets > 4096 || width > 4096) { set_error("CSF: lookup %u has an implausible shape (%u input sets x %u)", l, nsets, width); return false; }
-        if (!need(((uint64_t)nsets + 1) * (uint64_t)width)) { set_error("CSF: truncated lookup body"); return false; }
-        c.lookups[l].inputs.resize(nsets);
-        for (uint32_t s = 0; s < nsets; ++s) { c.lookups[l].inputs[s].assign(w + p, w + p + width); p += width; }
-        c.lookups[l].table.assign(w + p, w + p + width); p += width;
-    }
-    if (!need(2ull * (n_perm + n_aq + n_fq + n_iq))) { set_error("CSF: truncated tail"); return false; }
-    c.perm.resize(n_perm);
-    for (uint32_t i = 0; i < n_perm; ++i) { c.perm[i] = {w[p], w[p + 1]}; p += 2; }
-    auto rdq = [&](std::vector<std::array<int32_t, 2>> &q, uint32_t cnt) {
-        q.resize(cnt);
-        for (uint32_t i = 0; i < cnt; ++i) { q[i] = {(int32_t)w[p], (int32_t)w[p + 1]}; p += 2; }
-    };
-    rdq(c.advq, n_aq); rdq(c.fixq, n_fq); rdq(c.instq, n_iq);
-    for (auto &nd : c.nodes) {
-        if (nd[0] > N_SCALED) { set_error("CSF: bad node op"); return false; }
-    }
-    if (c.k < 1 || c.k > 26 || c.d < 3 || c.bf < 5) { set_error("CSF: bad k / degree / blinding factors"); return false; }
-    return true;
-}
-
-// parse a CSF blob and check it: node references point backwards, every column / challenge / constant index is in range
-static int32_t load_csf(const uint32_t *csf, uint64_t csf_words, Csf &c) {
-    ZKB_ARG(csf != nullptr);
-    if (!parse_csf(csf, csf_words, c)) return ZKB_ERR_ARG;
-    for (size_t i = 0; i < c.nodes.size(); ++i) {
-        const auto &nd = c.nodes[i];
-        bool ok = true;
-        switch (nd[0]) {
-        case N_CONST: ok = nd[1] < c.consts.size(); break;
-        case N_FIXED: ok = nd[1] < c.nf; break;
-        case N_ADVICE: ok = nd[1] < c.na; break;
-        case N_INSTANCE: ok = nd[1] < c.ni; break;
-        case N_CHALLENGE: ok = nd[1] < c.nch; break;
-        case N_NEG: ok = nd[1] < i; break;
-        case N_ADD: case N_MUL: ok = nd[1] < i && nd[2] < i; break;
-        case N_SCALED: ok = nd[1] < i && nd[2] < c.consts.size(); break;
-        }
-        if (!ok) { set_error("CSF: node %zu has an out-of-range operand", i); return ZKB_ERR_ARG; }
-    }
-    auto in_nodes = [&](uint32_t v) { return v < c.nodes.size(); };
-    for (auto g : c.gates) if (!in_nodes(g)) { set_error("CSF: gate references a missing node"); return ZKB_ERR_ARG; }
-    for (auto &lk : c.lookups) {
-        if (lk.inputs.empty() || lk.table.empty()) { set_error("CSF: empty lookup"); return ZKB_ERR_ARG; }
-        for (auto &inp : lk.inputs) for (auto v : inp) if (!in_nodes(v)) { set_error("CSF: lookup references a missing node"); return ZKB_ERR_ARG; }
-        for (auto v : lk.table) if (!in_nodes(v)) { set_error("CSF: lookup references a missing node"); return ZKB_ERR_ARG; }
-    }
-    for (auto &pc : c.perm) {
-        const uint32_t lim = pc[0] == N_FIXED ? c.nf : pc[0] == N_ADVICE ? c.na : pc[0] == N_INSTANCE ? c.ni : 0;
-        if (pc[1] >= lim) { set_error("CSF: permutation column out of range"); return ZKB_ERR_ARG; }
-    }
-    // queries: column in range, rotation representable in the interpreter's 16-bit field (also for expression nodes)
-    auto chkq = [&](const std::vector<std::array<int32_t, 2>> &q, uint32_t lim, const char *what) {
-        for (auto &e : q) {
-            if (e[0] < 0 || (uint32_t)e[0] >= lim) { set_error("CSF: %s query references column %d of %u", what, e[0], lim); return false; }
-            if (e[1] < -32767 || e[1] > 32767) { set_error("CSF: %s query rotation %d does not fit 16 bits", what, e[1]); return false; }
-        }
-        return true;
-    };
-    if (!chkq(c.advq, c.na, "advice") || !chkq(c.fixq, c.nf, "fixed") || !chkq(c.instq, c.ni, "instance")) return ZKB_ERR_ARG;
-    for (auto &nd : c.nodes) {
-        if (nd[0] == N_FIXED || nd[0] == N_ADVICE || nd[0] == N_INSTANCE) {
-            const int32_t rot = (int32_t)nd[2];
-            if (rot < -32767 || rot > 32767) { set_error("CSF: node rotation %d does not fit 16 bits", rot); return ZKB_ERR_ARG; }
-        }
-    }
-    if ((uint64_t)c.nf + c.na + c.ni + c.perm.size() + 1 >= 65536) { set_error("CSF: more than 65535 column slots"); return ZKB_ERR_ARG; }
-    for (uint32_t ph : c.adv_phase) if (ph >= c.nphases) { set_error("CSF: advice phase out of range"); return ZKB_ERR_ARG; }
-    for (uint32_t ph : c.ch_phase) if (ph >= c.nphases) { set_error("CSF: challenge phase out of range"); return ZKB_ERR_ARG; }
-    return ZKB_OK;
-}
-
-// The column slots of the interpreter's tables, in the one order every table uses:
-//   [fixed | advice | instance | sigma | X | l_0 | l_last | l_blind | z | phi | m]
-// The callers of the interpreter entry points pass the prefix [fixed | advice | instance].  A proof's value-domain table (lookup
-// compression, permutation products) is the prefix up to X, with X = omega^i; its quotient table is all of it on a coset part, with
-// X = the identity polynomial.  Fixed, sigma, X, l_0, l_last and l_blind do not depend on the proof: the pk caches their coset values.
-struct SlotMap {
-    uint32_t fixed0 = 0, advice0 = 0, instance0 = 0, sigma0 = 0, x = 0, l0 = 0, l_last = 0, l_blind = 0, z0 = 0, phi0 = 0, m0 = 0, slots = 0;
-    SlotMap() = default;
-    SlotMap(const Csf &cs, uint32_t nsets)
-        : advice0(cs.nf), instance0(advice0 + cs.na), sigma0(instance0 + cs.ni), x(sigma0 + (uint32_t)cs.perm.size()), l0(x + 1), l_last(x + 2),
-          l_blind(x + 3), z0(x + 4), phi0(z0 + nsets), m0(phi0 + (uint32_t)cs.lookups.size()), slots(m0 + (uint32_t)cs.lookups.size()) {}
-    // slot of a permutation column (kind, index)
-    uint32_t perm(const std::array<uint32_t, 2> &c) const { return c[0] == N_FIXED ? fixed0 + c[1] : c[0] == N_ADVICE ? advice0 + c[1] : instance0 + c[1]; }
-};
-// t[first + i] = cols[i]
-static void put_columns(std::vector<Fr *> &t, uint32_t first, const std::vector<Fr *> &cols) { std::copy(cols.begin(), cols.end(), t.begin() + first); }
 
 // ---------------------------------------------------------------------------------------------------------- small kernels
 __global__ void set_one_kernel(Fr *a, uint64_t idx) { fp_store(a + idx, Fr::one()); }
@@ -195,42 +60,7 @@ __global__ void interleave_rows_kernel(const Fr *__restrict__ slab, const uint32
     fp_store(out + idx, fp_load(slab + ((uint64_t)rows[j] << log_n) + i));
 }
 
-// ---- multiplicities of the mv-lookup: open-addressing hash table keyed by the 32-byte compressed table value --------
-__device__ __forceinline__ uint32_t key_hash(const Fr &k) {
-    uint32_t h = 0x9e3779b9u;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { h ^= k.l[i]; h *= 0x85ebca6bu; h ^= h >> 13; }
-    return h;
-}
-__global__ void m_insert_kernel(const Fr *__restrict__ t, uint32_t usable, uint32_t *slots, uint32_t mask) {
-    const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x;
-    if (tid >= usable) return;
-    const uint32_t i = usable - 1 - tid;  // descending row order: the winning (last) duplicate tends to arrive first
-    const Fr key = fp_load(t + i);
-    uint32_t h = key_hash(key) & mask;
-    while (true) {
-        const uint32_t s = atomicCAS(&slots[h], 0u, i + 1);
-        if (s == 0) return;
-        if (fp_load(t + (s - 1)) == key) {   // BTreeMap collect(): the last duplicate table row wins
-            if (s < i + 1) atomicMax(&slots[h], i + 1);
-            return;
-        }
-        h = (h + 1) & mask;
-    }
-}
-constexpr uint32_t NOT_IN_TABLE = 0xffffffffu;
-// the table row holding input row i's value, or NOT_IN_TABLE
-__device__ __forceinline__ uint32_t m_probe(const Fr *__restrict__ f, uint32_t i, const Fr *__restrict__ t, const uint32_t *__restrict__ slots,
-                                            uint32_t mask) {
-    const Fr key = fp_load(f + i);
-    uint32_t h = key_hash(key) & mask;
-    while (true) {
-        const uint32_t s = slots[h];
-        if (s == 0) return NOT_IN_TABLE;
-        if (fp_load(t + (s - 1)) == key) return s - 1;
-        h = (h + 1) & mask;
-    }
-}
+// ---- multiplicities of the mv-lookup: input rows counted per table row through the table's hash set (lookup.cuh) -----
 __global__ void m_count_kernel(const Fr *__restrict__ f, const Fr *__restrict__ t, uint32_t usable, const uint32_t *__restrict__ slots,
                                uint32_t mask, uint32_t *counts, int *err) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -243,15 +73,6 @@ __global__ void m_count_kernel(const Fr *__restrict__ f, const Fr *__restrict__ 
     const uint32_t peers = __match_any_sync(0xffffffffu, target);
     if (target != NOT_IN_TABLE && (threadIdx.x & 31) == (uint32_t)(__ffs(peers) - 1)) atomicAdd(&counts[target], (uint32_t)__popc(peers));
 }
-// witness check: the same probe as m_count_kernel, but one bit per row (word i / 32 by __ballot_sync, one writer per word) saying
-// "input row i < usable is not in the table"; launched over all words of the bitmap, rows >= usable vote 0
-__global__ void m_member_kernel(const Fr *__restrict__ f, const Fr *__restrict__ t, uint32_t usable, const uint32_t *__restrict__ slots,
-                                uint32_t mask, uint32_t *__restrict__ bits, uint32_t words) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    const bool missing = i < usable && m_probe(f, i, t, slots, mask) == NOT_IN_TABLE;
-    const uint32_t b = __ballot_sync(0xffffffffu, missing);
-    if ((threadIdx.x & 31) == 0 && (i >> 5) < words) bits[i >> 5] = b;
-}
 __global__ void counts_to_fr_kernel(const uint32_t *__restrict__ counts, uint32_t n, Fr *__restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) fp_store(out + i, fp_from_u64<FrParams>(counts[i]));
@@ -259,12 +80,6 @@ __global__ void counts_to_fr_kernel(const uint32_t *__restrict__ counts, uint32_
 
 // ---------------------------------------------------------------------------------------------------------- helpers
 static Fr fr_from_u64(uint64_t v) { return fp_from_u64<FrParams>(v); }
-// the permutation argument's DELTA = 7^(2^28): column i of a permutation set is labelled by DELTA^i
-static Fr perm_delta() {
-    Fr d = fr_from_u64(7);
-    for (int i = 0; i < 28; ++i) d = fp_sqr(d);
-    return d;
-}
 static bool fr_less(const Fr &a, const Fr &b) {  // halo2curves Ord: canonical integer comparison
     Fr x = fp_to_canonical(a), y = fp_to_canonical(b);
     for (int i = 7; i >= 0; --i) {
@@ -303,16 +118,7 @@ struct zkb_pk {
 
 struct zkb_session {
     zkb_pk *pk = nullptr;
-    // 0: Blake2bWrite<_, G1Affine, Challenge255<_>> (benches), 1: snark-verifier-sdk PoseidonTranscript (gen_snark_shplonk),
-    // 2: snark-verifier EvmTranscript over Keccak-256 (gen_evm_proof_shplonk), 3: the CALLER's transcript through zkb_transcript_vtable
-    // (create_proof's generic `T: TranscriptWrite`: the shim forwards the four operations to the Rust object it was handed)
-    int tkind = 0;
-    zkb_transcript_vtable vt{};
-    int32_t cb_error = 0;   // first non-zero return of a caller callback (checked after every stage)
-    Blake2b tr{"Halo2-Transcript"};
-    PoseidonSponge pos;
-    std::vector<uint8_t> evm_buf;
-    std::vector<uint8_t> proof;
+    Transcript tr;   // its callback status is checked after every stage
     DevPool pool;
     std::vector<Fr *> inst_values, inst_polys, adv_values;
     // columns handed over ahead of their phase (zkb_prove_upload_advice): staged device copies, consumed by zkb_prove_advice_phase
@@ -323,114 +129,6 @@ struct zkb_session {
 };
 
 namespace zkb {
-
-// ---------------------------------------------------------------------------------------------------------- transcript
-// base-field coordinate (canonical limbs, < q) -> scalar-field element (x mod r), Montgomery form: snark-verifier's fe_to_fe
-static Fr fq_canonical_to_fr(const Fq &c) {
-    uint32_t v[8];
-    for (int i = 0; i < 8; ++i) v[i] = c.l[i];
-    bool ge = true;
-    for (int i = 7; i >= 0; --i) {
-        if (v[i] != FrParams::P(i)) { ge = v[i] > FrParams::P(i); break; }
-    }
-    if (ge) {  // q < 2r: one subtraction suffices
-        int64_t br = 0;
-        for (int i = 0; i < 8; ++i) { int64_t d = (int64_t)v[i] - FrParams::P(i) + br; v[i] = (uint32_t)d; br = d >> 32; }
-    }
-    Fr out;
-    for (int i = 0; i < 8; ++i) out.l[i] = v[i];
-    return fp_from_canonical(out);
-}
-// 32-byte big-endian image of a canonical field element (EvmTranscript absorbs and writes `to_repr()` reversed)
-template <class F>
-static void push_be32(std::vector<uint8_t> &dst, const F &canonical) {
-    const uint8_t *b = (const uint8_t *)canonical.l;
-    for (int i = 31; i >= 0; --i) dst.push_back(b[i]);
-}
-// Challenge255 squeeze of a Blake2b transcript: absorb the 0x00 prefix, then Fr::from_uniform_bytes of the 64-byte digest,
-// (lo + hi * 2^256) mod r, computed with Montgomery multiplications by R^2
-static Fr blake2b_challenge255(Blake2b &tr) {
-    const uint8_t pre = 0;
-    tr.update(&pre, 1);
-    uint8_t h[64];
-    tr.finalize_copy(h);
-    Fr lo, hi;
-    memcpy(lo.l, h, 32);
-    memcpy(hi.l, h + 32, 32);
-    const Fr r2 = Fr::r2();
-    return fp_add(fp_mul(lo, r2), fp_mul(fp_mul(hi, r2), r2));
-}
-static void tr_common_scalar(zkb_session *s, const Fr &v) {
-    if (s->tkind == 3) { const int32_t r = s->vt.common_scalar(s->vt.user, (const uint64_t *)v.l); if (r && !s->cb_error) s->cb_error = r; return; }
-    if (s->tkind == 1) { s->pos.update(v); return; }
-    if (s->tkind == 2) { push_be32(s->evm_buf, fp_to_canonical(v)); return; }
-    const uint8_t pre = 2;
-    Fr c = fp_to_canonical(v);
-    s->tr.update(&pre, 1);
-    s->tr.update(c.l, 32);
-}
-static void tr_write_scalar(zkb_session *s, const Fr &v) {
-    if (s->tkind == 3) { const int32_t r = s->vt.write_scalar(s->vt.user, (const uint64_t *)v.l); if (r && !s->cb_error) s->cb_error = r; return; }
-    tr_common_scalar(s, v);
-    Fr c = fp_to_canonical(v);
-    if (s->tkind == 2) { push_be32(s->proof, c); return; }
-    const uint8_t *b = (const uint8_t *)c.l;
-    s->proof.insert(s->proof.end(), b, b + 32);
-}
-static int32_t tr_write_point(zkb_session *s, const G1Affine &p) {
-    if (p.is_identity()) { set_error("cannot write points at infinity to the transcript"); return ZKB_ERR_STATE; }
-    if (s->tkind == 3) {
-        const int32_t r = s->vt.write_point(s->vt.user, (const uint64_t *)&p);
-        if (r) { set_error("the caller's transcript refused a point (callback returned %d)", r); if (!s->cb_error) s->cb_error = r; return ZKB_ERR_STATE; }
-        return ZKB_OK;
-    }
-    Fq x = fp_to_canonical(p.x), y = fp_to_canonical(p.y);
-    if (s->tkind == 2) {  // absorbed and written uncompressed: x || y, big-endian
-        push_be32(s->evm_buf, x); push_be32(s->evm_buf, y);
-        push_be32(s->proof, x); push_be32(s->proof, y);
-        return ZKB_OK;
-    }
-    if (s->tkind == 1) {
-        s->pos.update(fq_canonical_to_fr(x));
-        s->pos.update(fq_canonical_to_fr(y));
-    } else {
-        const uint8_t pre = 1;
-        s->tr.update(&pre, 1);
-        s->tr.update(x.l, 32);
-        s->tr.update(y.l, 32);
-    }
-    uint8_t comp[32];
-    g1_compress(p, comp);
-    s->proof.insert(s->proof.end(), comp, comp + 32);
-    return ZKB_OK;
-}
-static Fr tr_squeeze(zkb_session *s) {
-    if (s->tkind == 3) {
-        Fr c = Fr::zero();
-        const int32_t r = s->vt.squeeze_challenge(s->vt.user, (uint64_t *)c.l);
-        if (r && !s->cb_error) s->cb_error = r;
-        return c;
-    }
-    if (s->tkind == 1) return s->pos.squeeze();
-    if (s->tkind == 2) {
-        // hash the buffer (plus a 0x01 byte when it holds just the previous digest), keep the digest as the new buffer,
-        // challenge = digest as a big-endian integer mod r
-        if (s->evm_buf.size() == 32) s->evm_buf.push_back(1);
-        uint8_t h[32];
-        keccak256(s->evm_buf.data(), s->evm_buf.size(), h);
-        s->evm_buf.assign(h, h + 32);
-        Fr v;
-        uint8_t *b = (uint8_t *)v.l;
-        for (int i = 0; i < 32; ++i) b[i] = h[31 - i];
-        return fp_mul(v, Fr::r2());  // Montgomery multiply reduces any 256-bit value: v * R^2 / R = v R mod r
-    }
-    return blake2b_challenge255(s->tr);
-}
-// first failure a caller's transcript callback reported (callbacks run inside the transcript operations, which return nothing)
-static int32_t callback_status(const zkb_session *s) {
-    if (s->cb_error) { set_error("the caller's transcript callback failed (%d)", s->cb_error); return ZKB_ERR_STATE; }
-    return ZKB_OK;
-}
 
 // ---------------------------------------------------------------------------------------------------------- basis changes
 static int32_t lagrange_to_coeff(zkb_pk *pk, const Fr *values, Fr *poly, cudaStream_t st) {
@@ -527,47 +225,10 @@ static int32_t commit_many(zkb_pk *pk, const std::vector<Fr *> &cols, int basis,
 static int32_t commit_write(zkb_session *s, const std::vector<Fr *> &cols, int basis, cudaStream_t st) {
     std::vector<G1Affine> cms;
     ZKB_TRY(commit_many(s->pk, cols, basis, cms, st));
-    for (auto &cm : cms) ZKB_TRY(tr_write_point(s, cm));
+    for (auto &cm : cms) ZKB_TRY(s->tr.write_point(cm));
     return ZKB_OK;
 }
 
-// program bundle uploaded to the device
-struct DeviceProgram {
-    Instr *code = nullptr;
-    uint32_t ncode = 0;
-    int nregs = 0;
-    Fr *consts = nullptr;
-};
-static int32_t upload_program(DevPool &pool, const ProgramBuilder &pb, const ExprBuilder &eb, DeviceProgram &dp, cudaStream_t st) {
-    dp.ncode = (uint32_t)pb.code.size();
-    dp.nregs = pb.max_regs_used;
-    ZKB_TRY(pool.alloc(pb.code.size() * sizeof(Instr) + 8, (void **)&dp.code));
-    ZKB_TRY(pool.alloc(eb.consts.size() * sizeof(Fr) + 32, (void **)&dp.consts));
-    ZKB_CUDA(cudaMemcpyAsync(dp.code, pb.code.data(), pb.code.size() * sizeof(Instr), cudaMemcpyHostToDevice, st));
-    ZKB_CUDA(cudaMemcpyAsync(dp.consts, eb.consts.data(), eb.consts.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
-    ZKB_CUDA(cudaStreamSynchronize(st));  // host vectors may die after return
-    return ZKB_OK;
-}
-template <class T>
-static int32_t upload_table(DevPool &pool, const std::vector<T *> &host, T ***dev, cudaStream_t st) {
-    ZKB_TRY(pool.alloc(host.size() * sizeof(T *) + 8, (void **)dev));
-    ZKB_CUDA(cudaMemcpyAsync(*dev, host.data(), host.size() * sizeof(T *), cudaMemcpyHostToDevice, st));
-    ZKB_CUDA(cudaStreamSynchronize(st));
-    return ZKB_OK;
-}
-// one program whose root i is STOREd to outs[i], uploaded with its output table and run over the 2^log_n rows of the d_cols table
-static int32_t run_store_program(zkb_ctx *ctx, uint32_t log_n, DevPool &pool, ExprBuilder &eb, const std::vector<uint32_t> &roots,
-                                 const std::vector<Fr *> &outs, const Fr *const *d_cols, const std::string &what, cudaStream_t st) {
-    ProgramBuilder pb(eb);
-    std::vector<ProgramBuilder::Root> stores;
-    for (size_t i = 0; i < roots.size(); ++i) stores.push_back({roots[i], ProgramBuilder::STORE, (uint32_t)i});
-    if (!pb.scope(stores)) { set_error("%s: %s", what.c_str(), pb.error.c_str()); return ZKB_ERR_ARG; }
-    DeviceProgram dp;
-    ZKB_TRY(upload_program(pool, pb, eb, dp, st));
-    Fr **d_outs = nullptr;
-    ZKB_TRY(upload_table(pool, outs, &d_outs, st));
-    return expr_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, d_outs, log_n, 1, 0, st);
-}
 // out (+)= sum_i coefs[i] * polys[i] over n coefficients.  `coefs` is copied asynchronously: keep it alive until the stream is synchronised.
 static int32_t lincomb(zkb_pk *pk, DevPool &pool, const std::vector<Fr *> &polys, const std::vector<Fr> &coefs, Fr *out, bool accumulate, cudaStream_t st) {
     Fr **d_p = nullptr;
@@ -576,76 +237,6 @@ static int32_t lincomb(zkb_pk *pk, DevPool &pool, const std::vector<Fr *> &polys
     ZKB_TRY(pool.fr(coefs.size(), &d_c));
     ZKB_CUDA(cudaMemcpyAsync(d_c, coefs.data(), coefs.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
     return lincomb_device(pk->ctx, d_p, d_c, (uint32_t)polys.size(), pk->n, out, accumulate, st);
-}
-
-// translate CSF nodes into ExprBuilder nodes
-static uint32_t translate(const Csf &cs, uint32_t node, ExprBuilder &eb, const SlotMap &sm, const std::vector<Fr> &challenges, std::vector<int64_t> &memo) {
-    if (memo[node] >= 0) return (uint32_t)memo[node];
-    const auto &nd = cs.nodes[node];
-    uint32_t r = 0;
-    switch (nd[0]) {
-    case N_CONST: r = eb.constant(cs.consts[nd[1]]); break;
-    case N_FIXED: r = eb.col(sm.fixed0 + nd[1], (int32_t)nd[2]); break;
-    case N_ADVICE: r = eb.col(sm.advice0 + nd[1], (int32_t)nd[2]); break;
-    case N_INSTANCE: r = eb.col(sm.instance0 + nd[1], (int32_t)nd[2]); break;
-    case N_CHALLENGE: r = eb.constant(challenges[nd[1]]); break;
-    case N_NEG: r = eb.neg(translate(cs, nd[1], eb, sm, challenges, memo)); break;
-    case N_ADD: { uint32_t a = translate(cs, nd[1], eb, sm, challenges, memo), b = translate(cs, nd[2], eb, sm, challenges, memo); r = eb.add(a, b); } break;
-    case N_MUL: { uint32_t a = translate(cs, nd[1], eb, sm, challenges, memo), b = translate(cs, nd[2], eb, sm, challenges, memo); r = eb.mul(a, b); } break;
-    case N_SCALED: { uint32_t a = translate(cs, nd[1], eb, sm, challenges, memo); r = eb.mul(a, eb.constant(cs.consts[nd[2]])); } break;
-    }
-    memo[node] = r;
-    return r;
-}
-// compressed = fold(exprs, acc * theta + e), first term taken as is (0 * theta + e0 == e0)
-static uint32_t compress_exprs(const Csf &cs, const std::vector<uint32_t> &exprs, ExprBuilder &eb, const SlotMap &sm, const std::vector<Fr> &ch,
-                               std::vector<int64_t> &memo, const Fr &theta) {
-    uint32_t acc = translate(cs, exprs[0], eb, sm, ch, memo);
-    for (size_t i = 1; i < exprs.size(); ++i) acc = eb.add(eb.mul(acc, eb.constant(theta)), translate(cs, exprs[i], eb, sm, ch, memo));
-    return acc;
-}
-// lookup l's compressed input sets into f[j] and its compressed table into t, over the 2^k rows of the d_cols table
-static int32_t lookup_compress(zkb_ctx *ctx, const Csf &cs, size_t l, const SlotMap &sm, const std::vector<Fr> &ch, const Fr &theta, DevPool &pool,
-                               const Fr *const *d_cols, std::vector<Fr *> f, Fr *t, cudaStream_t st) {
-    const CsfLookup &lk = cs.lookups[l];
-    ExprBuilder eb;
-    std::vector<int64_t> memo(cs.nodes.size(), -1);
-    std::vector<uint32_t> roots;
-    for (auto &inp : lk.inputs) roots.push_back(compress_exprs(cs, inp, eb, sm, ch, memo, theta));
-    roots.push_back(compress_exprs(cs, lk.table, eb, sm, ch, memo, theta));
-    f.push_back(t);
-    return run_store_program(ctx, cs.k, pool, eb, roots, f, d_cols, "lookup " + std::to_string(l), st);
-}
-// the hash set of table t's usable rows that m_count_kernel / m_member_kernel probe: the smallest power of two >= 2 usable slots,
-// cleared, then m_insert_kernel.  `slots` is allocated when null and otherwise reused (its size depends on `usable` only).
-static int32_t table_hash_set(zkb_ctx *ctx, DevPool &pool, const Fr *t, uint32_t usable, uint32_t *&slots, uint32_t &mask, cudaStream_t st) {
-    uint32_t tsize = 1;
-    while (tsize < 2 * usable) tsize <<= 1;
-    if (!slots) ZKB_TRY(pool.alloc((size_t)tsize * 4, (void **)&slots));
-    mask = tsize - 1;
-    ZKB_CUDA(cudaMemsetAsync(slots, 0, (size_t)tsize * 4, st));
-    if (usable) {   // the witness check takes circuits too small to have usable rows
-        m_insert_kernel<<<(usable + 255) / 256, 256, 0, st>>>(t, usable, slots, mask);
-        ctx->launches++;
-    }
-    return ZKB_OK;
-}
-
-constexpr uint32_t NO_NODE = 0xffffffffu;
-// permutation/prover.rs: the factors of set si over its columns j, multiplied left to right onto num (v_j + beta delta^j X + gamma) and
-// den (v_j + beta sigma_j + gamma); a product given as NO_NODE starts from its first factor.  X is slot sm.x in both domains.
-static void perm_set_products(const Csf &cs, const SlotMap &sm, uint32_t chunk, uint32_t si, const Fr &beta, const Fr &gamma, ExprBuilder &eb,
-                              uint32_t &num, uint32_t &den) {
-    const Fr delta = perm_delta();
-    Fr delta_pow = fp_pow_u64(delta, (uint64_t)si * chunk);
-    for (uint32_t j = si * chunk; j < std::min<size_t>((si + 1) * chunk, cs.perm.size()); ++j) {
-        const uint32_t v = eb.col(sm.perm(cs.perm[j]), 0);
-        const uint32_t dterm = eb.add(eb.add(v, eb.mul(eb.col(sm.sigma0 + j, 0), eb.constant(beta))), eb.constant(gamma));
-        const uint32_t nterm = eb.add(eb.add(v, eb.mul(eb.col(sm.x, 0), eb.constant(fp_mul(beta, delta_pow)))), eb.constant(gamma));
-        den = den == NO_NODE ? dterm : eb.mul(den, dterm);
-        num = num == NO_NODE ? nterm : eb.mul(num, nterm);
-        delta_pow = fp_mul(delta_pow, delta);
-    }
 }
 
 }  // namespace zkb
@@ -854,81 +445,6 @@ extern "C" int32_t zkb_pk_sigma_read(zkb_pk *pk, uint32_t column, uint64_t *out_
     return ZKB_OK;
 }
 
-// ---- host-only transcript primitives (no device needed): let the CPU test-suite pin the two hashers of the proving session ----
-// absorb n Fr elements (Montgomery) into a fresh Poseidon sponge (PoseidonTranscript::common_scalar) and squeeze one challenge
-extern "C" int32_t zkb_poseidon_hash_host(const uint64_t *inputs, uint64_t n, uint64_t out[4]) {
-    ZKB_ARG(out && (inputs || n == 0));
-    PoseidonSponge sp;
-    for (uint64_t i = 0; i < n; ++i) {
-        Fr v;
-        memcpy(v.l, inputs + 4 * i, 32);
-        sp.update(v);
-    }
-    const Fr c = sp.squeeze();
-    memcpy(out, c.l, 32);
-    return ZKB_OK;
-}
-// Host-only: replay a scripted sequence of transcript operations through the session's own transcript code (no device work).
-// ops[i]: 0 = common_scalar, 1 = write_scalar, 2 = write_point, 3 = squeeze_challenge; operands are consumed in order (scalar:
-// 4 limbs, point: 8 limbs, Montgomery form); challenges are appended to `challenges` (4 limbs each).  Lets the CPU suite pin the
-// framing of every transcript kind against the oracle's transcripts.
-extern "C" int32_t zkb_transcript_script_host(int32_t kind, const uint8_t *ops, uint64_t n_ops, const uint64_t *operands, uint8_t *proof, uint64_t cap,
-                                              uint64_t *proof_len, uint64_t *challenges) {
-    ZKB_ARG(kind >= 0 && kind <= 2 && (ops || n_ops == 0) && proof_len);
-    zkb_session s;  // no pk, no device pool: only the transcript members are touched
-    s.tkind = kind;
-    const uint64_t *op = operands;
-    for (uint64_t i = 0; i < n_ops; ++i) {
-        switch (ops[i]) {
-            case 0:
-            case 1: {
-                ZKB_ARG(op);
-                Fr v;
-                memcpy(v.l, op, 32);
-                op += 4;
-                if (ops[i] == 0) tr_common_scalar(&s, v); else tr_write_scalar(&s, v);
-                break;
-            }
-            case 2: {
-                ZKB_ARG(op);
-                G1Affine p;
-                memcpy(&p, op, 64);
-                op += 8;
-                ZKB_TRY(tr_write_point(&s, p));
-                break;
-            }
-            case 3: {
-                ZKB_ARG(challenges);
-                const Fr c = tr_squeeze(&s);
-                memcpy(challenges, c.l, 32);
-                challenges += 4;
-                break;
-            }
-            default: ZKB_ARG(false);
-        }
-    }
-    *proof_len = s.proof.size();
-    if (proof) {
-        ZKB_ARG(cap >= s.proof.size());
-        if (!s.proof.empty()) memcpy(proof, s.proof.data(), s.proof.size());
-    }
-    return ZKB_OK;
-}
-extern "C" int32_t zkb_keccak256_host(const uint8_t *bytes, uint64_t len, uint8_t out[32]) {
-    ZKB_ARG(out && (bytes || len == 0));
-    keccak256(bytes, len, out);
-    return ZKB_OK;
-}
-// feed raw bytes to a fresh Blake2b("Halo2-Transcript") state and squeeze one Challenge255 (prefix 0x00, 64-byte digest mod r)
-extern "C" int32_t zkb_blake2b_challenge_host(const uint8_t *bytes, uint64_t len, uint64_t out[4]) {
-    ZKB_ARG(out && (bytes || len == 0));
-    Blake2b st("Halo2-Transcript");
-    if (len) st.update(bytes, len);
-    const Fr c = blake2b_challenge255(st);
-    memcpy(out, c.l, 32);
-    return ZKB_OK;
-}
-
 // VerifyingKey::write(SerdeFormat::Processed) (halo2_proofs plonk.rs): u32 BE k || u32 BE num_fixed || fixed commitments ||
 // permutation commitments, points compressed -- the layout of the reference fixture's `vk` (aggregator/data/batch-task.json:
 // 0x19, 4, 4 + 3 points = 232 B).  Commitments = commit_lagrange of the fixed / sigma columns (keygen.rs), batched MSMs.
@@ -969,39 +485,20 @@ extern "C" int32_t zkb_pk_destroy(zkb_pk *pk) {
 }
 
 // ================================================================================================ C ABI: proof session
-extern "C" int32_t zkb_prove_begin_ex(zkb_pk *pk, int32_t transcript_kind, const uint64_t transcript_repr[4], const uint64_t *const *instance_values,
-                                      const uint32_t *instance_lens, zkb_session **out);
-extern "C" int32_t zkb_prove_begin(zkb_pk *pk, const uint64_t transcript_repr[4], const uint64_t *const *instance_values, const uint32_t *instance_lens,
-                                   zkb_session **out) {
-    return zkb_prove_begin_ex(pk, 0, transcript_repr, instance_values, instance_lens, out);
-}
-static int32_t prove_begin_common(zkb_pk *pk, int32_t transcript_kind, const zkb_transcript_vtable *vt, const uint64_t transcript_repr[4],
-                                  const uint64_t *const *instance_values, const uint32_t *instance_lens, zkb_session **out);
-extern "C" int32_t zkb_prove_begin_ex(zkb_pk *pk, int32_t transcript_kind, const uint64_t transcript_repr[4], const uint64_t *const *instance_values,
-                                      const uint32_t *instance_lens, zkb_session **out) {
-    ZKB_ARG(transcript_kind >= 0 && transcript_kind <= 2);
-    return prove_begin_common(pk, transcript_kind, nullptr, transcript_repr, instance_values, instance_lens, out);
-}
-extern "C" int32_t zkb_prove_begin_cb(zkb_pk *pk, const zkb_transcript_vtable *vt, const uint64_t transcript_repr[4],
-                                      const uint64_t *const *instance_values, const uint32_t *instance_lens, zkb_session **out) {
-    ZKB_ARG(vt && vt->common_scalar && vt->write_scalar && vt->write_point && vt->squeeze_challenge);
-    return prove_begin_common(pk, 3, vt, transcript_repr, instance_values, instance_lens, out);
-}
-static int32_t prove_begin_common(zkb_pk *pk, int32_t transcript_kind, const zkb_transcript_vtable *vt, const uint64_t transcript_repr[4],
+static int32_t prove_begin_common(zkb_pk *pk, Transcript::Kind transcript_kind, const zkb_transcript_vtable *vt, const uint64_t transcript_repr[4],
                                   const uint64_t *const *instance_values, const uint32_t *instance_lens, zkb_session **out) {
     ZKB_ARG(pk && transcript_repr && out && (pk->cs.ni == 0 || (instance_values && instance_lens)));
     ZKB_CUDA(cudaSetDevice(pk->ctx->device));
     std::unique_ptr<zkb_session> s(new zkb_session());
     s->pk = pk;
-    s->tkind = transcript_kind;
-    if (vt) s->vt = *vt;
+    s->tr = Transcript(transcript_kind, vt);
     s->pool.ctx = pk->ctx;
     const Csf &cs = pk->cs;
     const uint64_t n = pk->n;
     cudaStream_t st = pk->ctx->stream;
     Fr repr;
     memcpy(repr.l, transcript_repr, 32);
-    tr_common_scalar(s.get(), repr);  // vk.hash_into(transcript)
+    s->tr.common_scalar(repr);  // vk.hash_into(transcript)
     s->inst_values.resize(cs.ni);
     s->inst_polys.resize(cs.ni);
     for (uint32_t c = 0; c < cs.ni; ++c) {
@@ -1012,7 +509,7 @@ static int32_t prove_begin_common(zkb_pk *pk, int32_t transcript_kind, const zkb
         for (uint32_t i = 0; i < instance_lens[c]; ++i) {  // KZG: QUERY_INSTANCE = false -> values are absorbed as scalars
             Fr v;
             memcpy(v.l, instance_values[c] + 4 * i, 32);
-            tr_common_scalar(s.get(), v);
+            s->tr.common_scalar(v);
         }
         if (instance_lens[c]) ZKB_CUDA(cudaMemcpyAsync(s->inst_values[c], instance_values[c], (size_t)instance_lens[c] * sizeof(Fr), cudaMemcpyHostToDevice, st));
         ZKB_TRY(lagrange_to_coeff(pk, s->inst_values[c], s->inst_polys[c], st));
@@ -1020,9 +517,24 @@ static int32_t prove_begin_common(zkb_pk *pk, int32_t transcript_kind, const zkb
     s->adv_values.assign(cs.na, nullptr);
     s->challenges.assign(cs.nch, Fr::zero());
     ZKB_CUDA(cudaStreamSynchronize(st));
-    ZKB_TRY(callback_status(s.get()));
+    ZKB_TRY(s->tr.status());
     *out = s.release();
     return ZKB_OK;
+}
+
+extern "C" int32_t zkb_prove_begin(zkb_pk *pk, const uint64_t transcript_repr[4], const uint64_t *const *instance_values, const uint32_t *instance_lens,
+                                   zkb_session **out) {
+    return zkb_prove_begin_ex(pk, Transcript::BLAKE2B, transcript_repr, instance_values, instance_lens, out);
+}
+extern "C" int32_t zkb_prove_begin_ex(zkb_pk *pk, int32_t transcript_kind, const uint64_t transcript_repr[4], const uint64_t *const *instance_values,
+                                      const uint32_t *instance_lens, zkb_session **out) {
+    ZKB_ARG(transcript_kind >= Transcript::BLAKE2B && transcript_kind <= Transcript::EVM);
+    return prove_begin_common(pk, (Transcript::Kind)transcript_kind, nullptr, transcript_repr, instance_values, instance_lens, out);
+}
+extern "C" int32_t zkb_prove_begin_cb(zkb_pk *pk, const zkb_transcript_vtable *vt, const uint64_t transcript_repr[4],
+                                      const uint64_t *const *instance_values, const uint32_t *instance_lens, zkb_session **out) {
+    ZKB_ARG(vt && vt->common_scalar && vt->write_scalar && vt->write_point && vt->squeeze_challenge);
+    return prove_begin_common(pk, Transcript::CALLER, vt, transcript_repr, instance_values, instance_lens, out);
 }
 
 // Witness-side overlap (SURVEY 8f row 4): `synthesize` assigns sub-circuit after sub-circuit (super_circuit.rs:714-806), so the columns
@@ -1093,12 +605,12 @@ extern "C" int32_t zkb_prove_advice_phase(zkb_session *s, uint32_t phase, const 
     ZKB_TRY(deal_gather(pk->ctx, deal, slab, n * sizeof(Fr), st));   // column data of the other ranks' blocks over NVLink
     for (uint32_t i = 0; i < cs.nch; ++i) {
         if (cs.ch_phase[i] == phase) {
-            s->challenges[i] = tr_squeeze(s);
+            s->challenges[i] = s->tr.squeeze();
             if (challenges_out) memcpy(challenges_out + 4 * i, s->challenges[i].l, 32);
         }
     }
     s->next_phase++;
-    return callback_status(s);
+    return s->tr.status();
 }
 
 extern "C" int32_t zkb_session_destroy(zkb_session *s) {
@@ -1170,7 +682,7 @@ static int32_t lookup_prepare(zkb_session *s, ProofState &ps) {
     const size_t nl = cs.lookups.size();
     cudaStream_t st = ctx->stream;
     DevPool &pool = s->pool;
-    ps.theta = tr_squeeze(s);
+    ps.theta = s->tr.squeeze();
     ps.lk_f.resize(nl);
     ps.lk_t.resize(nl);
     const Deal deal(ctx, nl);
@@ -1230,8 +742,8 @@ static int32_t permutation_commit(zkb_session *s, ProofState &ps, const uint64_t
     const Fr one = Fr::one();
     cudaStream_t st = ctx->stream;
     DevPool &pool = s->pool;
-    ps.beta = tr_squeeze(s);
-    ps.gamma = tr_squeeze(s);
+    ps.beta = s->tr.squeeze();
+    ps.gamma = s->tr.squeeze();
     // Multi-GPU: the sets are dealt.  Upstream chains them (z_i[0] = last value of z_{i-1}), which is sequential; here every set is
     // scanned from 1 and rescaled afterwards by c_i = product of the previous sets' last values -- the same field elements
     // (z_i = c_i * z'_i row by row), with only the nsets last values crossing the ranks before the columns are gathered.
@@ -1340,7 +852,7 @@ static int32_t vanishing_commit(zkb_session *s, ProofState &ps, const uint64_t *
     ZKB_TRY(s->pool.fr(pk->n, &ps.random_poly));
     ZKB_CUDA(cudaMemcpyAsync(ps.random_poly, random_poly_host, pk->n * sizeof(Fr), cudaMemcpyHostToDevice, st));
     ZKB_TRY(commit_write(s, {ps.random_poly}, BASIS_G, st));
-    ps.y = tr_squeeze(s);
+    ps.y = s->tr.squeeze();
     return ZKB_OK;
 }
 
@@ -1693,7 +1205,7 @@ static int32_t vanishing_construct(zkb_session *s, ProofState &ps) {
     ZKB_CUDA(cudaStreamSynchronize(st));   // `mn_inv` lives on the stack
     for (uint32_t i = 0; i < pk->qdeg; ++i) ps.h_pieces.push_back(ps.h_ext + (size_t)i * pk->n);
     ZKB_TRY(commit_write(s, ps.h_pieces, BASIS_G, st));
-    ps.x = tr_squeeze(s);
+    ps.x = s->tr.squeeze();
     return ZKB_OK;
 }
 
@@ -1775,7 +1287,7 @@ static int32_t evaluate_at_x(zkb_session *s, ProofState &ps) {
         }
         for (size_t t = 0; t < kv.second.size(); ++t) evals[kv.second[t]] = res[t];
     }
-    for (size_t i = 0; i < n_written; ++i) tr_write_scalar(s, evals[i]);
+    for (size_t i = 0; i < n_written; ++i) s->tr.write_scalar(evals[i]);
     for (size_t i = 0; i < reqs.size(); ++i) ps.eval_of[{reqs[i].poly_id, reqs[i].rot}] = evals[i];
 
     // (2) multiopen queries in prover.rs order
@@ -1828,7 +1340,7 @@ static int32_t shplonk(zkb_session *s, ProofState &ps) {
     const Fr one = Fr::one();
     cudaStream_t st = ctx->stream;
     DevPool &pool = s->pool;
-    const Fr sy = tr_squeeze(s);
+    const Fr sy = s->tr.squeeze();
     // construct_intermediate_sets
     struct Commit { int id; const Fr *poly; std::vector<int64_t> rots; };
     std::vector<Commit> cmap;
@@ -1849,7 +1361,7 @@ static int32_t shplonk(zkb_session *s, ProofState &ps) {
         if (it == rsets.end()) rsets.push_back({c.rots, {&c}});
         else it->comms.push_back(&c);
     }
-    const Fr sv = tr_squeeze(s);
+    const Fr sv = s->tr.squeeze();
     Fr *hx, *work, *work2, *d_small;
     ZKB_TRY(pool.fr(n, &hx));
     ZKB_TRY(pool.fr(n, &work));
@@ -1895,7 +1407,7 @@ static int32_t shplonk(zkb_session *s, ProofState &ps) {
         vpow = fp_mul(vpow, sv);
     }
     ZKB_TRY(commit_write(s, {hx}, BASIS_G, st));
-    const Fr su = tr_squeeze(s);
+    const Fr su = s->tr.squeeze();
     // L(X) = sum_i v^i z_i sum_j y^j (P_ij(X) - r_ij) - zt * h_x(X), scaled by 1/z_0, divided by (X - u)
     std::vector<Fr> super_pts;
     for (int64_t r : super_rots) super_pts.push_back(ps.point_of[r]);
@@ -1968,7 +1480,7 @@ static int32_t prove_finish_stages(zkb_session *s, const uint64_t *z_blinds, con
     trace.mark("evaluations");
     ZKB_TRY(shplonk(s, ps));
     trace.mark("shplonk");
-    ZKB_TRY(callback_status(s));
+    ZKB_TRY(s->tr.status());
     s->finished = true;
     return ZKB_OK;
 }
@@ -1988,11 +1500,12 @@ extern "C" int32_t zkb_prove_finish(zkb_session *s, const uint64_t *z_blinds, co
         ZKB_CUDA(cudaSetDevice(pk->ctx->device));
         ZKB_TRY(prove_finish_stages(s, z_blinds, phi_blinds, random_poly));
     }
-    *proof_len = s->proof.size();
+    const std::vector<uint8_t> &proof = s->tr.proof();
+    *proof_len = proof.size();
     if (proof_out) {
-        if (proof_cap < s->proof.size()) { set_error("zkb_prove_finish: buffer of %llu bytes, proof has %llu (kept in the session: call again)",
-                                                     (unsigned long long)proof_cap, (unsigned long long)s->proof.size()); return ZKB_ERR_ARG; }
-        memcpy(proof_out, s->proof.data(), s->proof.size());
+        if (proof_cap < proof.size()) { set_error("zkb_prove_finish: buffer of %llu bytes, proof has %llu (kept in the session: call again)",
+                                             (unsigned long long)proof_cap, (unsigned long long)proof.size()); return ZKB_ERR_ARG; }
+        memcpy(proof_out, proof.data(), proof.size());
     }
     return ZKB_OK;
 }
@@ -2006,8 +1519,7 @@ extern "C" int32_t zkb_prove_finish(zkb_session *s, const uint64_t *z_blinds, co
 static int32_t gate_program(const Csf &cs, const SlotMap &sm, int32_t mode, const uint64_t *challenges, const uint64_t y[4], const uint64_t scale[4],
                             ExprBuilder &eb, ProgramBuilder &pb) {
     ZKB_ARG(cs.nch == 0 || challenges);
-    std::vector<Fr> ch(cs.nch);
-    for (uint32_t i = 0; i < cs.nch; ++i) memcpy(ch[i].l, challenges + 4 * i, sizeof(Fr));
+    const std::vector<Fr> ch = host_challenges(challenges, cs.nch);
     std::vector<int64_t> memo(cs.nodes.size(), -1);
     if (mode == 0) {
         std::vector<ProgramBuilder::Root> roots;
@@ -2065,124 +1577,5 @@ extern "C" int32_t zkb_expr_program(const uint32_t *csf, uint64_t csf_words, int
     *ncode_out = pb.code.size();
     if (nregs_out) *nregs_out = (uint32_t)pb.max_regs_used;
     if (cap) memcpy(code_out, pb.code.data(), std::min<uint64_t>(cap, pb.code.size()) * sizeof(Instr));
-    return ZKB_OK;
-}
-
-// ================================================================================================ C ABI: witness check
-// MockProver::run + assert_satisfied on the device (semantics in zkb200.h): one bitmap per gate (the interpreter's flag build, one
-// CSE scope per gate), per lookup input set (compression as lookup_prepare computes it, the table in m_insert_kernel's hash table,
-// m_member_kernel) and for the copy list (check.cu), then exact counts and the first `cap` records (check_collect).
-extern "C" int32_t zkb_check_witness_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, const uint64_t *const *columns_dev,
-                                         const uint64_t *challenges, const uint64_t *theta, const uint32_t *copies_dev, uint64_t n_copies,
-                                         uint64_t *counts_out, zkb_check_record *records_out, uint32_t cap, uint32_t *n_records, void *stream) {
-    ZKB_ARG(ctx && csf && columns_dev && counts_out && n_records && (records_out || cap == 0) && (copies_dev || n_copies == 0));
-    ZKB_ARG(n_copies < (1ull << 32));
-    ZKB_CUDA(cudaSetDevice(ctx->device));
-    Csf cs;
-    ZKB_TRY(load_csf(csf, csf_words, cs));
-    if (cs.nch && !challenges) { set_error("zkb_check_witness_dev: the constraint system has %u challenges and none were given", cs.nch); return ZKB_ERR_ARG; }
-    for (size_t l = 0; l < cs.lookups.size(); ++l)
-        if (cs.lookups[l].table.size() > 1 && !theta) {
-            set_error("zkb_check_witness_dev: lookup %zu has width %zu and needs theta", l, cs.lookups[l].table.size());
-            return ZKB_ERR_ARG;
-        }
-    std::vector<Fr> ch(cs.nch);
-    for (uint32_t i = 0; i < cs.nch; ++i) memcpy(ch[i].l, challenges + 4 * i, sizeof(Fr));
-    Fr th = Fr::zero();
-    if (theta) memcpy(th.l, theta, sizeof(Fr));
-    cudaStream_t st = pick_stream(ctx, stream);
-    const uint32_t n = 1u << cs.k, words = (n + 31) / 32;
-    const uint32_t usable = n > cs.bf + 1 ? n - cs.bf - 1 : 0;
-    const SlotMap sm(cs, 0);   // the caller's columns are its [fixed | advice | instance] prefix
-    const std::vector<Fr *> cols((Fr *const *)columns_dev, (Fr *const *)columns_dev + sm.sigma0);
-    size_t nsets = 0, maxsets = 0;
-    for (auto &lk : cs.lookups) { nsets += lk.inputs.size(); maxsets = std::max(maxsets, lk.inputs.size()); }
-    const uint64_t copy_words = (n_copies + 31) / 32;
-    DevPool pool;
-    pool.ctx = ctx;
-    Fr **d_cols = nullptr;
-    uint32_t *bits = nullptr;
-    ZKB_TRY(upload_table(pool, cols, &d_cols, st));
-    ZKB_TRY(pool.alloc(((cs.gates.size() + nsets) * words + copy_words) * 4, (void **)&bits));
-    uint32_t *lk_bits = bits + cs.gates.size() * words, *copy_bits = lk_bits + nsets * words;
-    std::vector<CheckItem> items;
-
-    if (!cs.gates.empty()) {   // gates: one scope per gate, no selector folding
-        ProfScope ps_(ctx, PROF_CHECK_GATES, st);
-        ExprBuilder eb;
-        ProgramBuilder pb(eb);
-        std::vector<int64_t> memo(cs.nodes.size(), -1);
-        for (size_t g = 0; g < cs.gates.size(); ++g)
-            if (!pb.scope({{translate(cs, cs.gates[g], eb, sm, ch, memo), ProgramBuilder::FLAG, (uint32_t)g}})) {
-                set_error("gate %zu: %s", g, pb.error.c_str());
-                return ZKB_ERR_ARG;
-            }
-        DeviceProgram dp;
-        ZKB_TRY(upload_program(pool, pb, eb, dp, st));
-        ZKB_TRY(expr_flag_run_device(ctx, dp.code, dp.ncode, dp.nregs, d_cols, dp.consts, bits, words, cs.k, st));
-    }
-    for (size_t g = 0; g < cs.gates.size(); ++g) items.push_back({bits + g * words, words, 0, (uint32_t)g, 0, 0, 0});
-
-    if (nsets) {               // lookups, one argument at a time: compressed inputs and table, the table's hash set, membership bits
-        ProfScope ps_(ctx, PROF_CHECK_LOOKUPS, st);
-        std::vector<Fr *> bufs(maxsets + 1);
-        for (auto &b : bufs) ZKB_TRY(pool.fr(n, &b));
-        uint32_t *slots = nullptr, mask = 0;
-        uint32_t *out = lk_bits;
-        for (size_t l = 0; l < cs.lookups.size(); ++l) {
-            const size_t ns = cs.lookups[l].inputs.size();
-            ZKB_TRY(lookup_compress(ctx, cs, l, sm, ch, th, pool, d_cols, std::vector<Fr *>(bufs.begin(), bufs.begin() + ns), bufs[maxsets], st));
-            ZKB_TRY(table_hash_set(ctx, pool, bufs[maxsets], usable, slots, mask, st));
-            for (size_t j = 0; j < ns; ++j, out += words) {
-                m_member_kernel<<<(n + 255) / 256, 256, 0, st>>>(bufs[j], bufs[maxsets], usable, slots, mask, out, words);
-                ctx->launches++;
-                items.push_back({out, words, 1, (uint32_t)l, (uint32_t)j, 0, 0});
-            }
-            ZKB_CUDA(cudaGetLastError());
-        }
-    }
-
-    {                          // copies
-        ProfScope ps_(ctx, PROF_CHECK_COPIES, st);
-        std::vector<Fr *> pc;
-        for (auto &c : cs.perm) pc.push_back(cols[sm.perm(c)]);
-        Fr **d_pc = nullptr;
-        ZKB_TRY(upload_table(pool, pc, &d_pc, st));
-        uint64_t first_bad = 0;
-        ZKB_TRY(copy_flags_device(ctx, pool, copies_dev, n_copies, d_pc, (uint32_t)pc.size(), n, copy_bits, &first_bad, st));
-        if (first_bad != ~0ull) {
-            set_error("zkb_check_witness_dev: copy constraint %llu is out of range (column >= %zu or row >= %u)", (unsigned long long)first_bad,
-                      pc.size(), n);
-            return ZKB_ERR_ARG;
-        }
-    }
-    items.push_back({copy_bits, copy_words, 2, 0, 0, 0, 0});
-
-    ZKB_TRY(check_collect(ctx, pool, items, copies_dev, counts_out, records_out, cap, n_records, st));
-    // poisoned gate failures: an advice query of the gate reads a row >= usable at the failing row
-    std::vector<std::vector<int32_t>> adv_rots(cs.gates.size());
-    std::vector<bool> adv_rots_done(cs.gates.size(), false);
-    for (uint32_t i = 0; i < *n_records && records_out[i].kind == 0; ++i) {
-        zkb_check_record &r = records_out[i];
-        std::vector<int32_t> &rots = adv_rots[r.index];
-        if (!adv_rots_done[r.index]) {
-            std::vector<uint32_t> stack{cs.gates[r.index]};
-            std::vector<bool> seen(cs.nodes.size(), false);
-            while (!stack.empty()) {
-                const uint32_t v = stack.back();
-                stack.pop_back();
-                if (seen[v]) continue;
-                seen[v] = true;
-                const auto &nd = cs.nodes[v];
-                if (nd[0] == N_ADVICE) rots.push_back((int32_t)nd[2]);
-                else if (nd[0] == N_NEG || nd[0] == N_SCALED) stack.push_back(nd[1]);
-                else if (nd[0] == N_ADD || nd[0] == N_MUL) { stack.push_back(nd[1]); stack.push_back(nd[2]); }
-            }
-            adv_rots_done[r.index] = true;
-        }
-        r.sub = 0;
-        for (int32_t rot : rots)
-            if (((r.row + (uint32_t)rot) & (n - 1)) >= usable) { r.sub = 1; break; }
-    }
     return ZKB_OK;
 }
