@@ -9,7 +9,9 @@
 //   is ONE persistent kernel, TWO 256-thread CTAs per SM, each walking over TILES of 2048 elements (64 KB): a tile is C = 2048 / A
 //   adjacent columns of the Cooley-Tukey index split, i.e. C independent length-A transforms whose rows are C*32 contiguous bytes
 //   in HBM.  The two resident CTAs run out of phase, so while one waits for TMA data, converts layouts or streams results out, the
-//   other is in its multiplier-bound butterfly rounds: the integer-multiply pipe (the bound, see DESIGN.md) stays fed.  Per tile:
+//   other is in its multiplier-bound butterfly rounds: the integer-multiply pipe (the bound, see DESIGN.md) stays fed.  (One CTA
+//   per SM with 255 registers and a second data buffer removes every spill but leaves 8 warps per SM, too few to cover the
+//   multiply chains: measured slower, DESIGN.md section 3.1.)  Per tile:
 //     * the data tile is fetched by TMA (cp.async.bulk.tensor.2d through a per-column tensor map: box = 256 rows x 32 B;
 //       the contiguous sub-transforms of the last pass by cp.async.bulk), completion signalled on an mbarrier
 //       (complete_tx::bytes); the fetch of tile i+1 is issued the moment tile i's last result left shared memory;
@@ -23,8 +25,9 @@
 //       compile time and cost no multiply: (A/2) log2 A - (A - 1) + A/8 multiplies per transform instead of (A/2) log2 A;
 //     * two 16-byte planes with an XOR swizzle + one padding slot per column -> conflict-free 128-bit LDS/STS;
 //     * results leave through 32-byte streaming stores, C adjacent threads writing C*32 contiguous bytes.
-//   Scaling by 1/n (any caller scale) is folded into the last inter-pass table; zeta-coset scaling and an arbitrary
-//   per-element input scale are fused into the first / last register round.
+//   Scaling by 1/n (any caller scale) is folded into the last inter-pass table; zeta-coset scaling of the output is fused into
+//   the store phase, zeta-coset scaling and an arbitrary per-element scale of the input are applied in place to the freshly
+//   loaded tile of the first pass, one element per thread and step, before its first register round.
 #include "common.cuh"
 #include <string.h>
 #include <stdlib.h>
@@ -34,7 +37,7 @@
 namespace zkb {
 
 // Two 256-thread CTAs per SM on 2048-element tiles: a non-final pass takes 105 KB of shared memory per CTA (header + data tile
-// + twiddle ring + local twiddles), so two CTAs fit the 228 KB of an H100 SM.
+// + twiddle ring + local twiddles), so two CTAs fit the 228 KB of an H100 SM.  A second data tile per CTA does not fit.
 constexpr int NTT_TILE_BITS = 11;        // 2048 elements = 64 KB per tile
 constexpr int NTT_MAX_BITS = 11;         // largest in-CTA transform (final pass: no twiddle ring in shared memory)
 constexpr int NTT_PREF_INNER_BITS = 9;   // non-final passes: <= 8 KB of local twiddles next to the 32 KB twiddle ring -> two CTAs per SM
@@ -158,13 +161,34 @@ __device__ __forceinline__ Fr zeta_pow(int i) {  // i in {1,2}
     return z;
 }
 
+// First pass: the input scalings (ZETA^(i mod 3), then the per-element in_scale) applied in place on the TMA layout L0, one
+// element per step.  Fused into the first register round they held eight scale loads and products live next to the eight data
+// elements, which pushed the round past the register budget into local-memory spills.
+__device__ __forceinline__ void scale_input(uint8_t *dbuf, const PassArgs &p, const TileInfo &ti, uint32_t tid) {
+    const uint32_t a = p.a, elems = 1u << (a + p.log_c);
+    uint4 *q = reinterpret_cast<uint4 *>(dbuf);
+#pragma unroll 1
+    for (uint32_t e = tid; e < elems; e += NTT_THREADS) {
+        const uint32_t c = e >> a, r = e & ((1u << a) - 1);
+        const uint32_t idx = (r << p.log_inner) + ti.c0 + c;   // first pass: outer == 0
+        Fr v = ld_lin(dbuf, e);
+        if (p.coset_in) {
+            const uint32_t z = idx % 3;
+            if (z) v = fp_mul_lazy(v, zeta_pow(z));
+        }
+        if (p.has_in_scale) v = fp_mul_lazy(v, fp_load(p.in_scale + idx));
+        st_l1(q + 2 * e, q + 2 * e + 1, 0, v);
+    }
+    __syncthreads();
+}
+
 // R consecutive DIF stages (s .. s+R-1) on groups of 2^R elements held in registers: one shared-memory round trip and one
 // barrier per R stages.  Every thread owns 8 element slots per round (8 / 2^R groups).  FIRST: the inputs are read from the
-// TMA layout L0 (with the fused input scalings), then -- after a barrier, the conversion is in place -- written in L1.
+// TMA layout L0 (already scaled by scale_input), then -- after a barrier, the conversion is in place -- written in L1.
 // LAST (s + R == a): the group's elements are adjacent rows, so the twiddle exponents depend on the register index alone and the
 // unit twiddles (m & (d - 1)) == 0 are dropped at compile time.
 template <int R, bool FIRST, bool LAST>
-__device__ __forceinline__ void ntt_round(uint8_t *dbuf, const PassArgs &p, const TileInfo &ti, uint32_t s, const uint8_t *loc_sm, uint32_t tid) {
+__device__ __forceinline__ void ntt_round(uint8_t *dbuf, const PassArgs &p, uint32_t s, const uint8_t *loc_sm, uint32_t tid) {
     constexpr int E = 1 << R, NG = 8 / E;
     const uint32_t a = p.a, A = 1u << a;
     const uint32_t elems = 1u << (a + p.log_c);
@@ -208,24 +232,7 @@ __device__ __forceinline__ void ntt_round(uint8_t *dbuf, const PassArgs &p, cons
             else x[u * E + m] = ld_l1(lo, hi, c * (A + 1) + swz(r));
         }
     }
-    if (FIRST) {
-        if (p.coset_in || p.has_in_scale) {
-#pragma unroll
-            for (int u = 0; u < NG; ++u) {
-#pragma unroll
-                for (int m = 0; m < E; ++m) {
-                    const uint32_t r = rbase[u] + ((uint32_t)m << lq);
-                    const uint32_t idx = (r << p.log_inner) + ti.c0 + cbase[u];   // first pass: outer == 0
-                    if (p.coset_in) {
-                        const uint32_t z = idx % 3;
-                        if (z) x[u * E + m] = fp_mul_lazy(x[u * E + m], zeta_pow(z));
-                    }
-                    if (p.has_in_scale) x[u * E + m] = fp_mul_lazy(x[u * E + m], fp_load(p.in_scale + idx));
-                }
-            }
-        }
-        __syncthreads();  // every L0 read is done before the first L1 write (same bytes)
-    }
+    if (FIRST) __syncthreads();  // every L0 read is done before the first L1 write (same bytes)
 #pragma unroll
     for (int u = 0; u < NG; ++u) {
 #pragma unroll
@@ -328,47 +335,54 @@ __global__ void __launch_bounds__(NTT_THREADS, NTT_CTAS_PER_SM) ntt_tile_kernel(
     for (uint32_t it = 0; gt < p.total_tiles; ++it, gt += stride) {
         const TileInfo ti = decode_tile(p, gt);
         mbar_wait(bar_d, it & 1);
+        if (p.coset_in || p.has_in_scale) scale_input(d, p, ti, tid);
 
         // decimation in frequency: natural order in, bit-reversed order out (inside shared memory); radix-8 rounds in registers,
         // the short round (a mod 3 stages) first, so that the last one is a full radix-8 round with compile-time unit twiddles
         if (a == 0) {
-            ntt_round<0, true, false>(d, p, ti, 0, locbuf, tid);
+            ntt_round<0, true, false>(d, p, 0, locbuf, tid);
             __syncthreads();
         } else {
             const uint32_t r0 = a % 3 ? a % 3 : 3;
-            if (r0 == 1) ntt_round<1, true, false>(d, p, ti, 0, locbuf, tid);
-            else if (r0 == 2) ntt_round<2, true, false>(d, p, ti, 0, locbuf, tid);
-            else ntt_round<3, true, false>(d, p, ti, 0, locbuf, tid);
+            if (r0 == 1) ntt_round<1, true, false>(d, p, 0, locbuf, tid);
+            else if (r0 == 2) ntt_round<2, true, false>(d, p, 0, locbuf, tid);
+            else ntt_round<3, true, false>(d, p, 0, locbuf, tid);
             __syncthreads();
             uint32_t s = r0;
-            while (a - s > 3) { ntt_round<3, false, false>(d, p, ti, s, locbuf, tid); __syncthreads(); s += 3; }
-            if (a - s == 3) { ntt_round<3, false, true>(d, p, ti, s, locbuf, tid); __syncthreads(); }
+            while (a - s > 3) { ntt_round<3, false, false>(d, p, s, locbuf, tid); __syncthreads(); s += 3; }
+            if (a - s == 3) { ntt_round<3, false, true>(d, p, s, locbuf, tid); __syncthreads(); }
         }
 
         const uint4 *lo = reinterpret_cast<const uint4 *>(d);
         const uint4 *hi = lo + ((A + 1) << p.log_c);
         Fr *__restrict__ out = p.dst[ti.y];
         if (!p.is_final) {
-            // slot q of a column holds output k = bitrev(q); the staged table is [q][c] in exactly this order
-            for (uint32_t u = 0; u < nchunks; ++u, ++g_wait) {
-                const uint32_t slot = g_wait & 3u;
-                mbar_wait(bar_tw0 + 8 * slot, (g_wait >> 2) & 1u);
-                const uint32_t e = tid + u * NTT_THREADS;
-                if (tid < chunk_elems) {
-                    const uint32_t c = e & (C - 1), q = e >> p.log_c;
-                    const uint32_t k = __brev(q) >> (32 - a);   // a >= 1 in non-final passes
-                    const Fr v = fp_mul_lazy(ld_l1(lo, hi, c * (A + 1) + swz(q)), ld_lin(twring + slot * (NTT_TW_SLOT_ELEMS * 32u), tid));   // < 2p: the next pass takes it lazily
-                    const uint64_t oidx = ((((uint64_t)ti.outer << a) + k) << p.log_inner) + ti.c0 + c;
-                    fp_store_stream(out + oidx, v);
+            // slot q of a column holds output k = bitrev(q); the staged table is [q][c] in exactly this order.  Two ring slots are
+            // consumed per barrier and refilled after it, which leaves the other two (the next two chunks) in flight
+            const uint32_t per_sync = nchunks > 1 ? 2u : 1u;
+            for (uint32_t u = 0; u < nchunks; u += per_sync) {
+                for (uint32_t j = 0; j < per_sync; ++j, ++g_wait) {
+                    const uint32_t slot = g_wait & 3u;
+                    mbar_wait(bar_tw0 + 8 * slot, (g_wait >> 2) & 1u);
+                    const uint32_t e = tid + (u + j) * NTT_THREADS;
+                    if (tid < chunk_elems) {
+                        const uint32_t c = e & (C - 1), q = e >> p.log_c;
+                        const uint32_t k = __brev(q) >> (32 - a);   // a >= 1 in non-final passes
+                        const Fr v = fp_mul_lazy(ld_l1(lo, hi, c * (A + 1) + swz(q)), ld_lin(twring + slot * (NTT_TW_SLOT_ELEMS * 32u), tid));   // < 2p: the next pass takes it lazily
+                        const uint64_t oidx = ((((uint64_t)ti.outer << a) + k) << p.log_inner) + ti.c0 + c;
+                        fp_store_stream(out + oidx, v);
+                    }
                 }
-                // generic-proxy reads of this slot (and, after the last iteration, of the data buffer) are ordered before the
+                // generic-proxy reads of these slots (and, after the last iteration, of the data buffer) are ordered before the
                 // async-proxy (TMA) writes that reuse them
                 fence_proxy_async();
                 __syncthreads();
-                if (tid == 0 && is_gt < p.total_tiles) {
-                    issue_tw(p, is_gt, is_c, chunk_elems, smem_u32(twring) + (is_g & 3u) * (NTT_TW_SLOT_ELEMS * 32u), bar_tw0 + 8 * (is_g & 3u));
-                    ++is_g;
-                    if (++is_c == nchunks) { is_c = 0; is_gt += stride; }
+                if (tid == 0) {
+                    for (uint32_t j = 0; j < per_sync && is_gt < p.total_tiles; ++j) {
+                        issue_tw(p, is_gt, is_c, chunk_elems, smem_u32(twring) + (is_g & 3u) * (NTT_TW_SLOT_ELEMS * 32u), bar_tw0 + 8 * (is_g & 3u));
+                        ++is_g;
+                        if (++is_c == nchunks) { is_c = 0; is_gt += stride; }
+                    }
                 }
             }
         } else {
