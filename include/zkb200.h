@@ -182,6 +182,44 @@ ZKB_API int32_t zkb_field_unop_dev(zkb_ctx *ctx, int32_t field, int32_t op, cons
 /* Montgomery batch inversion (halo2 `BatchInvert` / batch_invert_assigned): out[i] = a[i]^-1, zeros stay zero. */
 ZKB_API int32_t zkb_fr_batch_invert_dev(zkb_ctx *ctx, const uint64_t *a, uint64_t *out, uint64_t n, void *stream);
 
+/* Test surface: one primitive of ff.cuh / g1.cuh applied to n records of raw operands.  Operands are NOT reduced or
+ * checked, so the lazy forms' wider input ranges can be reached.  in: n x arity x 4 u64, out: n x width x 4 u64.
+ * field: 0 = Fr, 1 = Fq (G1 ops need 1).  Values are the stored integers (Montgomery form for field elements); the contract
+ * is what each primitive is specified for -- outside it the output is unspecified.
+ *   op  primitive                  operands            contract (stored integers)                 output
+ *    0  fp_add                     a, b                < p                                        (a + b) mod p
+ *    1  fp_sub                     a, b                < p                                        (a - b) mod p
+ *    2  fp_neg                     a                   < p                                        (-a) mod p
+ *    3  fp_dbl                     a                   < p                                        2a mod p
+ *    4  fp_mul                     a, b                < p                                        a b / R mod p
+ *    5  fp_sqr                     a                   < p                                        a^2 / R mod p
+ *    6  fp_mul_add_mul             a, b, c, d          a, c <= p; b, d < p                        (a b + c d) / R mod p
+ *    7  fp_mul_sub_mul             a, b, c, d          a <= p; b, c, d < p                        (a b - c d) / R mod p
+ *    8  fp_mul_lazy                a, b                a < 4p and b < p, or a, b < 2p             the REDC value (a b + M p) / R < 2p
+ *    9  fp_add_lazy                a, b                < 2p                                       a + b, minus 2p if >= 2p: [0, 2p)
+ *   10  fp_sub_lazy                a, b                < 2p                                       a - b + 2p: (0, 4p)
+ *   11  fp_cond_sub<false>         x                   < 2p                                       x, minus p if >= p: [0, p)
+ *   12  fp_cond_sub<true>          x                   < 4p                                       x, minus 2p if >= 2p: [0, 2p)
+ *   13  fp_pow                     a, e                a < p; e any 256-bit integer               a^e (Montgomery), a^0 = one
+ *   14  fp_pow_u64                 a, e                a < p; e = limb 0 of the second operand    a^e (Montgomery)
+ *   15  fp_inv                     a                   < p                                        a^-1 (Montgomery); inv(0) = 0
+ *   16  fp_from_canonical          a                   < p                                        a R mod p
+ *   17  fp_to_canonical            a                   < p                                        a / R mod p
+ *   18  fp_from_u64                v                   limb 0, any u64                            v R mod p
+ *   32  g1_add_mixed               acc XYZZ, q affine  points in Fq (Montgomery)                  acc + q, XYZZ
+ *   33  g1_add                     acc XYZZ, q XYZZ                                               acc + q, XYZZ
+ *   34  g1_dbl                     XYZZ                                                           2P, XYZZ
+ *   35  g1_dbl_affine              affine                                                         2P, XYZZ
+ *   36  g1_to_affine               XYZZ                                                           affine, identity (0, 0)
+ *   37  g1_neg                     affine                                                         affine
+ *   38  G1Xyzz::from_affine        affine                                                         XYZZ (x, y, one, one), identity zeros
+ * R = 2^256; M = (-a b p^-1) mod R.  XYZZ is x = X / ZZ, y = Y / ZZZ with ZZ^3 = ZZZ^2, the identity when ZZ = 0.
+ * zkb_arith_probe_host runs the host-compiled branches of the same templates; the device-only ops 8 - 12 return ZKB_ERR_ARG
+ * there, as does an unknown op or a G1 op with field != 1 on either side.  Needs no CUDA device.                          */
+ZKB_API int32_t zkb_arith_probe_dev(zkb_ctx *ctx, int32_t field, int32_t op, const uint64_t *in_dev, uint64_t *out_dev,
+                                    uint64_t n, void *stream);
+ZKB_API int32_t zkb_arith_probe_host(int32_t field, int32_t op, const uint64_t *in, uint64_t *out, uint64_t n);
+
 /* ---- polynomial utilities around MSM/NTT (device buffers) ----------------------------------------------------
  * zkb_fr_powers_dev        out[i] = base^i
  * zkb_poly_eval_dev        halo2_proofs::arithmetic::eval_polynomial for `num_polys` polynomials (host array of device

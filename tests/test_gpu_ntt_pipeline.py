@@ -1,6 +1,7 @@
 """The NTT tile kernel's double-buffered tile walk, limb for limb against the oracle's best_fft: batches whose tile count leaves
 CTAs with an odd number of tiles (the buffer parity wraps), exactly one tile per CTA, fewer tiles than CTAs, the zeta coset on
-the input and on the output of 1-, 2- and 3-pass plans, and launches queued back to back on one stream into the same buffers."""
+the input and on the output of 1-, 2- and 3-pass plans, inputs at the top of the field, and launches queued back to back on one
+stream into the same buffers."""
 import numpy as np
 import pytest
 
@@ -30,11 +31,13 @@ def zeta_tables(oracle, n):
     return np.stack([one, zeta, zeta2])[idx], np.stack([one, zeta2, zeta])[idx]
 
 
-def check_batch(A, oracle, log_n, count, seed, inverse=False, coset_zeta=0):
+def check_batch(A, oracle, log_n, count, seed, inverse=False, coset_zeta=0, cols=None):
     from zkb200 import poly as Pz
     n = 1 << log_n
     w, wi = A.root_of_unity(log_n)
-    cols = [rand_field(n, seed + i) for i in range(count)]
+    if cols is None:
+        cols = [rand_field(n, seed + i) for i in range(count)]
+    count = len(cols)
     scale = None
     if inverse:
         scale = oracle.fr_inv(oracle.fr_from_canonical(np.array([[n, 0, 0, 0]], dtype=np.uint64)))[0]
@@ -76,6 +79,25 @@ def test_fewer_tiles_than_ctas(A, oracle, log_n):
 def test_coset_in_and_out(A, oracle, log_n):
     check_batch(A, oracle, log_n, 2, 7600 + log_n, coset_zeta=1)
     check_batch(A, oracle, log_n, 2, 7700 + log_n, inverse=True, coset_zeta=2)
+
+
+@pytest.mark.parametrize("log_n", [10, 16, 21])   # 1-, 2- and 3-pass plans
+def test_extreme_inputs(A, oracle, log_n):
+    """inputs that drive the lazy (< 2p) butterflies to the top of their ranges: every element p - 1, 0 and p - 1 alternating, and
+    p - 1 only at index 0 and at n - 1 (stored integers), through the forward transform, the inverse with the fused 1/n, and the zeta
+    coset on the input and on the output"""
+    n = 1 << log_n
+    top = np.array(P.limbs(P.R_MOD - 1), dtype=np.uint64)
+    full = np.repeat(top[None], n, axis=0)
+    alt = full.copy()
+    alt[0::2] = 0
+    ends = np.zeros((n, 4), dtype=np.uint64)
+    ends[0] = ends[-1] = top
+    cols = [full, alt, ends]
+    check_batch(A, oracle, log_n, 0, 0, cols=cols)
+    check_batch(A, oracle, log_n, 0, 0, inverse=True, cols=cols)
+    check_batch(A, oracle, log_n, 0, 0, coset_zeta=1, cols=cols)
+    check_batch(A, oracle, log_n, 0, 0, inverse=True, coset_zeta=2, cols=cols)
 
 
 @pytest.mark.parametrize("log_n", [11, 15, 21])

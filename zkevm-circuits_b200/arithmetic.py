@@ -4,7 +4,8 @@ halo2_proofs 1.1.0 @ e5ddf67 src/arithmetic.rs: `best_fft(a, omega, log_n)`, `be
 Array conventions (halo2curves in-memory layout): Fr/Fq = 4 little-endian u64 limbs in Montgomery form.
   host   : numpy uint64 arrays, shape (n, 4) for scalars, (n, 8) for G1Affine
   device : torch int64 CUDA tensors of the same shapes (torch has no uint64 arithmetic; only storage is used)
-Every function drives the CUDA kernels through the C ABI; nothing here computes on the CPU.
+Every function drives the CUDA kernels through the C ABI; nothing here computes on the CPU (arith_probe_host runs the library's
+own host-compiled primitives, for tests).
 """
 import ctypes
 import numpy as np
@@ -183,6 +184,35 @@ def fr_batch_invert_dev(a, ctx=None):
     ctx = ctx or default_context(a.device.index)
     out = torch.empty_like(a)
     check(ctx.lib.zkb_fr_batch_invert_dev(ctx.handle, _vp(a.data_ptr()), _vp(out.data_ptr()), a.shape[0], _cur_stream()))
+    return out
+
+
+# ---- primitive probe (test surface of ff.cuh / g1.cuh, include/zkb200.h zkb_arith_probe_*) --------------------------------
+# op -> (field elements read per record, field elements written per record)
+PROBE_SHAPE = {0: (2, 1), 1: (2, 1), 2: (1, 1), 3: (1, 1), 4: (2, 1), 5: (1, 1), 6: (4, 1), 7: (4, 1), 8: (2, 1), 9: (2, 1),
+               10: (2, 1), 11: (1, 1), 12: (1, 1), 13: (2, 1), 14: (2, 1), 15: (1, 1), 16: (1, 1), 17: (1, 1), 18: (1, 1),
+               32: (6, 4), 33: (8, 4), 34: (4, 4), 35: (2, 4), 36: (4, 2), 37: (2, 2), 38: (2, 4)}
+
+
+def arith_probe_dev(field, op, a, ctx=None):
+    """Primitive `op` on every record of a (torch int64 CUDA tensor (n, arity * 4)) -> (n, width * 4), torch's current stream."""
+    import torch
+    ctx = ctx or default_context(a.device.index)
+    arity, width = PROBE_SHAPE[op]
+    assert a.is_cuda and a.is_contiguous() and a.dim() == 2 and a.shape[1] == 4 * arity
+    out = torch.empty((a.shape[0], 4 * width), dtype=torch.int64, device=a.device)
+    check(ctx.lib.zkb_arith_probe_dev(ctx.handle, field, op, _vp(a.data_ptr()), _vp(out.data_ptr()), a.shape[0], _cur_stream()))
+    return out
+
+
+def arith_probe_host(field, op, a):
+    """The host-compiled branch of the same primitive: a numpy uint64 (n, arity * 4) -> (n, width * 4).  Needs no device."""
+    from .lib import load_library
+    arity, width = PROBE_SHAPE[op]
+    a = np.ascontiguousarray(a, dtype=np.uint64)
+    assert a.ndim == 2 and a.shape[1] == 4 * arity
+    out = np.zeros((a.shape[0], 4 * width), dtype=np.uint64)
+    check(load_library().zkb_arith_probe_host(field, op, _np_ptr(a), _np_ptr(out), a.shape[0]))
     return out
 
 

@@ -250,6 +250,7 @@ FF_D void chain_stray_mad_nc(uint32_t &x0, uint32_t stray, uint32_t &c0, uint32_
 // REDUCE = false: the final conditional subtraction is skipped and the result is only guaranteed < 2p ("lazy" form, used by the NTT
 // butterflies).  Bounds (word-serial CIOS): the running value stays < a + p and the result is < a*b/R + p, so with R = 2^256 > 4p the
 // lazy product of a < 4p (first operand, the one that feeds the multiply chains) and b < p is < 2p and nothing overflows 8 limbs.
+// The host branch has no lazy form: it always makes the final subtraction (no host code multiplies lazily).
 template <class PR, bool REDUCE>
 FF_HD Fp<PR> fp_mul_t(const Fp<PR> &a, const Fp<PR> &b) {
     Fp<PR> r;
@@ -342,7 +343,7 @@ FF_HD Fp<PR> fp_mul_t(const Fp<PR> &a, const Fp<PR> &b) {
 
 template <class PR>
 FF_HD Fp<PR> fp_mul(const Fp<PR> &a, const Fp<PR> &b) { return fp_mul_t<PR, true>(a, b); }
-// a < 4p, b < p (or both < 2p)  ->  a*b/R mod p as a representative < 2p
+// a < 4p, b < p (or both < 2p)  ->  the REDC value (a b + M p) / R, M = -a b p^-1 mod R: a representative of a*b/R mod p below 2p
 template <class PR>
 FF_HD Fp<PR> fp_mul_lazy(const Fp<PR> &a, const Fp<PR> &b) { return fp_mul_t<PR, false>(a, b); }
 
@@ -642,7 +643,8 @@ FF_HD Fp<PR> fp_mul_add_mul(const Fp<PR> &a, const Fp<PR> &b, const Fp<PR> &c, c
 #endif
 }
 
-// a * b - c * d with one reduction, as a * b + (p - c) * d: p - c is in (0, p], so T < 2p^2 as for the sum
+// a * b - c * d with one reduction (a <= p; b, c, d < p), as a * b + (p - c) * d: p - c is in (0, p] (p itself for c = 0), so
+// T < 2p^2 as for the sum
 template <class PR>
 FF_HD Fp<PR> fp_mul_sub_mul(const Fp<PR> &a, const Fp<PR> &b, const Fp<PR> &c, const Fp<PR> &d) {
 #if defined(__CUDA_ARCH__)
@@ -749,7 +751,7 @@ __device__ __forceinline__ Fp<PR> fp_cond_sub(const Fp<PR> &x) {
 }
 #endif
 
-// a^e, e given as 8 x u32 little-endian (plain integer)
+// a^e, e given as 8 x u32 little-endian (plain integer: any 256-bit value, bit 255 included); a^0 = one, also for a = 0
 template <class PR>
 FF_HD Fp<PR> fp_pow(const Fp<PR> &a, const uint32_t e[8]) {
     Fp<PR> acc = Fp<PR>::one(), base = a;

@@ -59,6 +59,8 @@ SIGNATURES = {
     "zkb_field_binop_dev": (ctypes.c_int32, [_vp, ctypes.c_int32, ctypes.c_int32, _vp, _vp, _vp, ctypes.c_uint64, _vp]),
     "zkb_field_unop_dev": (ctypes.c_int32, [_vp, ctypes.c_int32, ctypes.c_int32, _vp, _vp, ctypes.c_uint64, _vp]),
     "zkb_fr_batch_invert_dev": (ctypes.c_int32, [_vp, _vp, _vp, ctypes.c_uint64, _vp]),
+    "zkb_arith_probe_dev": (ctypes.c_int32, [_vp, ctypes.c_int32, ctypes.c_int32, _vp, _vp, ctypes.c_uint64, _vp]),
+    "zkb_arith_probe_host": (ctypes.c_int32, [ctypes.c_int32, ctypes.c_int32, _vp, _vp, ctypes.c_uint64]),
     "zkb_fr_powers_dev": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, _vp, _vp]),
     "zkb_poly_eval_dev": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint32, ctypes.c_uint64, _vp, _vp, _vp]),
     "zkb_fr_prefix_product_dev": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, _vp, _vp, _vp]),
