@@ -224,6 +224,7 @@ ZKB_API int32_t zkb_arith_probe_host(int32_t field, int32_t op, const uint64_t *
  * zkb_fr_powers_dev        out[i] = base^i
  * zkb_poly_eval_dev        halo2_proofs::arithmetic::eval_polynomial for `num_polys` polynomials (host array of device
  *                          pointers, n coefficients each) at one point x; results (Montgomery) to out_host; synchronises.
+ *                          num_polys <= 65535, else ZKB_ERR_ARG before any launch.
  * zkb_fr_prefix_product_dev / _sum_dev   out[0] = init, out[i+1] = out[i] (*|+) in[i]  (n outputs; the running product z of
  *                          permutation/prover.rs and the running sum phi of mv_lookup/prover.rs)
  * zkb_kate_division_dev    halo2_proofs::arithmetic::kate_division: q = (a(X) - a(u)) / (X - u); q has n entries, q[n-1] = 0 */
@@ -337,6 +338,20 @@ ZKB_API int32_t zkb_expr_eval_dev(zkb_ctx *ctx, const uint32_t *csf, uint64_t cs
  * NULL) receives the register count that picks the kernel build.  For instruction counts (scripts/expr_program_stats.py).    */
 ZKB_API int32_t zkb_expr_program(const uint32_t *csf, uint64_t csf_words, int32_t mode, const uint64_t *challenges, const uint64_t y[4],
                                  const uint64_t scale[4], uint64_t *code_out, uint64_t cap, uint64_t *ncode_out, uint32_t *nregs_out);
+/* Test surface: the mv-lookup multiplicities m exactly as zkb_prove_finish computes them (mv_lookup/prover.rs prepare), over caller
+ * buffers of already-compressed values (Montgomery Fr, compared as stored bytes).  inputs_dev: HOST array of n_sets device pointers, n
+ * elements each; table_dev: n elements.  m_out_dev[r] (n Fr, Montgomery) = the number of input rows i < usable over all sets whose value
+ * the table holds at row r, where r is the LAST table row < usable with that value (BTreeMap collect()); every other row, rows >= usable
+ * included, is zero.  Input rows >= usable are ignored.  *unsatisfied = 1 when an input row < usable is not among the table rows < usable,
+ * else 0 (the prover's "unsatisfied witness" error; the rows that are found are still counted).  The table's hash set has
+ * n_slots = the smallest power of two >= 2 usable u32 slots: 0 = empty, otherwise table row + 1, probed linearly from
+ * key_hash(value) & (n_slots - 1) (csrc/lookup.cuh).  Which slot of its probe run a key lands in depends on the insertion schedule, so
+ * the slots may differ between calls while m does not.  The first min(slots_cap, n_slots) slots go to slots_out (host, may be NULL when
+ * slots_cap is 0) and n_slots to *n_slots (may be NULL).  ZKB_ERR_ARG before any launch unless 0 < usable < n <= 2^31 and
+ * n_sets >= 1.  Synchronises `stream`.                                                                                          */
+ZKB_API int32_t zkb_lookup_multiplicities_dev(zkb_ctx *ctx, const uint64_t *const *inputs_dev, uint32_t n_sets, const uint64_t *table_dev, uint64_t n,
+                                              uint32_t usable, uint64_t *m_out_dev, int32_t *unsatisfied, uint32_t *slots_out, uint64_t slots_cap,
+                                              uint64_t *n_slots, void *stream);
 /* Witness check (halo2 MockProver::run + verify / assert_satisfied_par, without region information): which constraints of a CSF
  * fail on caller columns, row by row, before any proof is attempted.  A failure is what the verifier would reject:
  *   gate g          g(row) != 0 on ALL n rows (rotation r reads row (row + r) mod n): the quotient needs every gate to vanish on

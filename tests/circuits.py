@@ -159,7 +159,9 @@ class ThinCompressionShape:
         cs.fixed_queries = [(1, 0), (0, 0), (2, 0), (3, 0)]
         return cs
 
-    def __init__(self, k, seed=0, n_instance=6):
+    def __init__(self, k, seed=0, n_instance=6, table=None):
+        """table: optional usable -> (m, 4) uint64 array of extra table values in the stored (Montgomery) form; they follow the T small
+        values, a few of them repeat at later rows and one past the usable rows, and the range-checked cells draw from the whole table."""
         rnd = random.Random(seed)
         self.k, self.n = k, 1 << k
         n = self.n
@@ -172,6 +174,14 @@ class ThinCompressionShape:
         T = 1 << max(2, k - 2)
         fixed = [[0] * n for _ in range(4)]
         for j in range(T): fixed[0][j] = j
+        if table is not None:
+            extra = [P.from_mont(P.from_limbs(v), R) for v in table(usable)]
+            dups = [extra[rnd.randrange(len(extra))] for _ in range(max(1, len(extra) // 8))]
+            assert T + len(extra) + len(dups) <= usable
+            fixed[0][T:T + len(extra)] = extra
+            fixed[0][T + len(extra):T + len(extra) + len(dups)] = dups
+            fixed[0][usable] = extra[0]
+            T = T + len(extra) + len(dups)          # the range-checked cells below draw from every table row set so far
         self.instances = [[rnd.randrange(R) for _ in range(n_instance)]]
         A = [rnd.randrange(T) for _ in range(n)]          # default: small values (valid lookup inputs)
         copies = []
@@ -189,7 +199,7 @@ class ThinCompressionShape:
                 r += 4
             else:                                          # a range-checked cell
                 fixed[3][r] = 1
-                A[r] = rnd.randrange(T)
+                A[r] = fixed[0][rnd.randrange(T)]
                 r += 1
         for _ in range(usable // 8):
             i, j = rnd.randrange(usable), rnd.randrange(usable)

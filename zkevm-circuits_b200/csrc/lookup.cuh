@@ -1,5 +1,5 @@
 // lookup.cuh -- the mv-lookup's compressed values and the hash set of a compressed table, shared by the prover's multiplicities
-// (m_count_kernel, prover.cu) and the witness check's membership flags (m_member_kernel, check.cu).  The set is an open-addressing
+// (lookup_multiplicities, lookup.cu) and the witness check's membership flags (m_member_kernel, check.cu).  The set is an open-addressing
 // hash table keyed by the 32-byte compressed table value.
 #pragma once
 #include "csf.cuh"
@@ -32,5 +32,11 @@ int32_t lookup_compress(zkb_ctx *ctx, const Csf &cs, size_t l, const SlotMap &sm
 // the hash set of table t's usable rows that m_probe searches: the smallest power of two >= 2 usable slots, cleared, then filled.
 // `slots` is allocated when null and otherwise reused (its size depends on `usable` only).
 int32_t table_hash_set(zkb_ctx *ctx, DevPool &pool, const Fr *t, uint32_t usable, uint32_t *&slots, uint32_t &mask, cudaStream_t st);
+// mv_lookup/prover.rs multiplicities: m_out[r] (n Fr, Montgomery) = the number of input rows i < usable, over the n_sets compressed
+// input sets f[j] (a host array of device pointers), whose value is the one table t holds at row r, where r is the LAST row < usable
+// holding that value (BTreeMap collect()); rows >= usable are zero.  Builds t's hash set into `slots` / `mask` (table_hash_set) and
+// sets *unsatisfied when an input row < usable is not in the table.  Synchronises st.
+int32_t lookup_multiplicities(zkb_ctx *ctx, DevPool &pool, const Fr *const *f, size_t n_sets, const Fr *t, uint64_t n, uint32_t usable, Fr *m_out,
+                              uint32_t *&slots, uint32_t &mask, bool *unsatisfied, cudaStream_t st);
 
 }  // namespace zkb

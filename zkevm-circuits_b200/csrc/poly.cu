@@ -369,6 +369,7 @@ extern "C" int32_t zkb_fr_powers_dev(zkb_ctx *ctx, const uint64_t base[4], uint6
 extern "C" int32_t zkb_poly_eval_dev(zkb_ctx *ctx, const uint64_t *const *polys_dev, uint32_t num_polys, uint64_t n, const uint64_t x[4],
                                      uint64_t *out_host, void *stream) {
     ZKB_ARG(ctx && polys_dev && x && out_host && n > 0);
+    ZKB_ARG(num_polys <= 65535);   // one grid row (gridDim.y) per polynomial
     cudaStream_t st = pick_stream(ctx, stream);
     Fr **tbl = nullptr;
     ZKB_TRY(scratch_get(ctx, SCR_MISC, (size_t)num_polys * sizeof(Fr *), (void **)&tbl));

@@ -60,24 +60,6 @@ __global__ void interleave_rows_kernel(const Fr *__restrict__ slab, const uint32
     fp_store(out + idx, fp_load(slab + ((uint64_t)rows[j] << log_n) + i));
 }
 
-// ---- multiplicities of the mv-lookup: input rows counted per table row through the table's hash set (lookup.cuh) -----
-__global__ void m_count_kernel(const Fr *__restrict__ f, const Fr *__restrict__ t, uint32_t usable, const uint32_t *__restrict__ slots,
-                               uint32_t mask, uint32_t *counts, int *err) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    uint32_t target = NOT_IN_TABLE;
-    if (i < usable) {
-        target = m_probe(f, i, t, slots, mask);
-        if (target == NOT_IN_TABLE) atomicExch(err, 1);  // input not in table: unsatisfied lookup
-    }
-    // most rows of a zkEVM lookup hit the same few table rows (selector off -> the all-zero row): aggregate per warp
-    const uint32_t peers = __match_any_sync(0xffffffffu, target);
-    if (target != NOT_IN_TABLE && (threadIdx.x & 31) == (uint32_t)(__ffs(peers) - 1)) atomicAdd(&counts[target], (uint32_t)__popc(peers));
-}
-__global__ void counts_to_fr_kernel(const uint32_t *__restrict__ counts, uint32_t n, Fr *__restrict__ out) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) fp_store(out + i, fp_from_u64<FrParams>(counts[i]));
-}
-
 // ---------------------------------------------------------------------------------------------------------- helpers
 static Fr fr_from_u64(uint64_t v) { return fp_from_u64<FrParams>(v); }
 static bool fr_less(const Fr &a, const Fr &b) {  // halo2curves Ord: canonical integer comparison
@@ -697,19 +679,9 @@ static int32_t lookup_prepare(zkb_session *s, ProofState &ps) {
         for (auto &f : ps.lk_f[l]) ZKB_TRY(pool.fr(n, &f));
         ZKB_TRY(pool.fr(n, &ps.lk_t[l]));
         ZKB_TRY(lookup_compress(ctx, cs, l, pk->sm, s->challenges, ps.theta, pool, ps.d_vcols, ps.lk_f[l], ps.lk_t[l], st));
-        // multiplicities over the usable rows
-        ZKB_TRY(table_hash_set(ctx, pool, ps.lk_t[l], usable, slots, mask, st));
-        uint32_t *counts = nullptr;
-        ZKB_TRY(pool.alloc((size_t)n * 4 + 16, (void **)&counts));
-        int *d_err = (int *)(counts + n);
-        ZKB_CUDA(cudaMemsetAsync(counts, 0, (size_t)n * 4 + 16, st));
-        for (size_t j = 0; j < ns; ++j) m_count_kernel<<<(usable + 255) / 256, 256, 0, st>>>(ps.lk_f[l][j], ps.lk_t[l], usable, slots, mask, counts, d_err);
-        counts_to_fr_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(counts, (uint32_t)n, ps.lk_m[l]);
-        ctx->launches += 1 + ns;
-        int herr = 0;
-        ZKB_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, st));
-        ZKB_CUDA(cudaStreamSynchronize(st));
-        if (herr) {
+        bool unsatisfied = false;
+        ZKB_TRY(lookup_multiplicities(ctx, pool, ps.lk_f[l].data(), ns, ps.lk_t[l], n, usable, ps.lk_m[l], slots, mask, &unsatisfied, st));
+        if (unsatisfied) {
             set_error("lookup %zu: an input row is not in the table (unsatisfied witness)", l);
             if (!deal.on) return ZKB_ERR_ARG;
             lookup_errors++;   // multi-GPU: every rank must learn about it before anyone leaves the collective sequence

@@ -86,6 +86,8 @@ SIGNATURES = {
                                           ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint32)]),
     "zkb_check_witness_dev": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, _vp, _vp, _vp, _vp, ctypes.c_uint64, _vp, _vp, ctypes.c_uint32,
                                                ctypes.POINTER(ctypes.c_uint32), _vp]),
+    "zkb_lookup_multiplicities_dev": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint32, _vp, ctypes.c_uint64, ctypes.c_uint32, _vp,
+                                                       ctypes.POINTER(ctypes.c_int32), _vp, ctypes.c_uint64, ctypes.POINTER(ctypes.c_uint64), _vp]),
     "zkb_prove_begin": (ctypes.c_int32, [_vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
     "zkb_prove_begin_ex": (ctypes.c_int32, [_vp, ctypes.c_int32, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
     "zkb_prove_begin_cb": (ctypes.c_int32, [_vp, _vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),

@@ -143,6 +143,33 @@ def expr_eval(cs, columns, mode=0, challenges=(), y=None, scale=None, out=None, 
     return outs, int(nregs.value)
 
 
+def lookup_multiplicities(inputs, table, usable, slots=False, ctx=None):
+    """The prover's mv-lookup multiplicities (zkb_lookup_multiplicities_dev) on torch's current stream.
+
+    inputs: list of torch int64 CUDA tensors (n, 4), compressed input sets; table: the compressed table (n, 4).  Returns
+    (m: (n, 4) CUDA tensor, Montgomery Fr; unsatisfied: bool), plus the table's hash-set slots as a numpy uint32 array when `slots`."""
+    import torch
+    from .arithmetic import _cur_stream
+    ctx = ctx or default_context(table.device.index)
+    n = table.shape[0]
+    assert all(t.is_cuda and t.dtype == torch.int64 and t.is_contiguous() and t.shape == (n, 4) for t in list(inputs) + [table])
+    m = torch.empty((n, 4), dtype=torch.int64, device=table.device)
+    itbl = (ctypes.c_void_p * max(1, len(inputs)))(*[t.data_ptr() for t in inputs])
+    unsat = ctypes.c_int32(0)
+    nslots = ctypes.c_uint64(0)
+    tsize = 1
+    while tsize < 2 * usable:
+        tsize <<= 1
+    sl = np.zeros(tsize if slots else 0, dtype=np.uint32)
+    check(ctx.lib.zkb_lookup_multiplicities_dev(ctx.handle, ctypes.cast(itbl, _vp), len(inputs), _vp(table.data_ptr()), n, int(usable),
+                                                _vp(m.data_ptr()), ctypes.byref(unsat), _vp(sl.ctypes.data) if slots else None, sl.size,
+                                                ctypes.byref(nslots), _cur_stream()))
+    if slots:
+        assert nslots.value == tsize
+        return m, bool(unsat.value), sl
+    return m, bool(unsat.value)
+
+
 def expr_program(cs, mode=0, challenges=(), y=None, scale=None):
     """Host only: the interpreter program expr_eval would run (zkb_expr_program), as (uint64 array, one word per instruction:
     op | dst << 8 | a << 16 | b << 24 | imm << 32, register count)."""
