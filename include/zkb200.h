@@ -101,8 +101,8 @@ ZKB_API uint64_t zkb_msm_last_adds(const zkb_ctx *ctx);
 /* Bucket-reduction levels beyond the first that the last MSM actually executed (decided on the device, no host round trip). */
 ZKB_API uint32_t zkb_msm_last_levels(const zkb_ctx *ctx);
 
-/* out[i] = [scalars[i]] * base, affine outputs (device buffers).  Used for ParamsKZG::setup / unsafe_setup_with_s
- * (g[i] = [s^i] G) and to synthesise distinct benchmark bases.                                                  */
+/* out[i] = [scalars[i]] * base, affine outputs (device buffers).  A plain double-and-add with one inversion per point: the
+ * independent reference zkb_srs_setup_dev is tested against, and the source of distinct benchmark bases.  Not the setup path. */
 ZKB_API int32_t zkb_g1_fixed_base_mul_dev(zkb_ctx *ctx, const uint64_t base_affine_host[8], const uint64_t *scalars_dev,
                                   uint64_t n, uint64_t *out_affine_dev, void *stream);
 
@@ -131,6 +131,23 @@ ZKB_API int32_t zkb_srs_commit_host(zkb_srs *srs, int32_t basis, const uint64_t 
                                     uint8_t *out_compressed);
 ZKB_API int32_t zkb_srs_commit_batch_dev(zkb_srs *srs, int32_t basis, const uint64_t *const *scalar_cols_dev, uint32_t batch, uint64_t n,
                                          uint64_t *out_affine, void *stream);
+
+/* ---- SRS generation: ParamsKZG::unsafe_setup_with_s (and setup / new, whose s the caller draws) --------------------------------------
+ * zkb_srs_setup_dev   g[i] = [s^i] G1 and g_lagrange[i] = [L_i(s)] G1 for i < 2^k, L_i(s) = w^i (s^n - 1) / (n (s - w^i)), G1 = (1, 2),
+ *                     written as 2^k x 64 B affine points to two device buffers (16-byte aligned).  s is a HOST Montgomery Fr whose
+ *                     stored integer is < r; k <= 28.  A violation returns ZKB_ERR_ARG before any launch and leaves the outputs
+ *                     untouched.  Scratch (2 * 2^k x 32 B of scalars and the comb table) comes from the context's block cache and is
+ *                     returned before the call returns; synchronises `stream`.  The same inputs give the same bytes on every run.
+ *                     Deviation from upstream: when s^n = 1 (s = w^j, e.g. s = 1 or s = r - 1), upstream's invert().unwrap() panics;
+ *                     here g_lagrange is the true Lagrange basis, g_lagrange[j] = G1 and every other entry (0, 0), which equals
+ *                     what downsize's group iFFT derives from g.
+ * zkb_srs_setup_dev reads ZKB_SETUP_WINDOW_BITS (6, 7, 8, 10, 12 default) and ZKB_SETUP_TABLE_SMEM (1: comb table in shared memory,
+ *                     c <= 7) to select a comb variant; every variant computes the same bytes.
+ * zkb_g2_setup_host   g2_out = the G2 generator, s_g2_out = [s] g2, raw 128-byte points in the layout of zkb_g2_*_host (x.c0, x.c1,
+ *                     y.c0, y.c1, Montgomery; identity = zeros).  Same rule for s; host only, no device needed.                        */
+ZKB_API int32_t zkb_srs_setup_dev(zkb_ctx *ctx, uint32_t k, const uint64_t s[4], uint64_t *g_out_dev, uint64_t *g_lagrange_out_dev,
+                                  void *stream);
+ZKB_API int32_t zkb_g2_setup_host(const uint64_t s[4], uint64_t g2_out[16], uint64_t s_g2_out[16]);
 
 /* ---- params file points: ParamsKZG::read_custom / write_custom (halo2_proofs src/poly/kzg/commitment.rs) --------------------------
  * A params file is 4 B k (u32 LE) | g: 2^k G1 | g_lagrange: 2^k G1 | g2 | s_g2, each point in the SerdeFormat the caller names (the

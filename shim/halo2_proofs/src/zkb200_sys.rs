@@ -1,4 +1,4 @@
-//! Raw bindings of include/zkb200.h (ABI version 1.1).  Field elements and points cross as `*const u64` / `*mut u64`:
+//! Raw bindings of include/zkb200.h (ABI version 1.5).  Field elements and points cross as `*const u64` / `*mut u64`:
 //! halo2curves' `Fr`, `Fq` are `#[repr(transparent)]` over `[u64; 4]` (Montgomery form) and `G1Affine` is `{ x: Fq, y: Fq }`, so
 //! `slice.as_ptr() as *const u64` needs no conversion (layout checked against the reference fixture in tests/test_oracle_golden.py).
 #![allow(non_camel_case_types)]
@@ -51,6 +51,13 @@ extern "C" {
     pub fn zkb_g1_encode(ctx: *mut zkb_ctx, format: i32, in_affine: *const u64, n: u64, out: *mut u8, stream: *mut c_void) -> i32;
     pub fn zkb_g2_decode_host(format: i32, input: *const u8, out: *mut u64, status: *mut i32) -> i32;
     pub fn zkb_g2_encode_host(format: i32, input: *const u64, out: *mut u8) -> i32;
+    // ParamsKZG::setup / unsafe_setup_with_s / new (s: Montgomery Fr < r; outputs 2^k G1Affine each, device buffers)
+    pub fn zkb_srs_setup_dev(ctx: *mut zkb_ctx, k: u32, s: *const u64, g_out_dev: *mut u64, g_lagrange_out_dev: *mut u64,
+                             stream: *mut c_void) -> i32;
+    pub fn zkb_g2_setup_host(s: *const u64, g2_out: *mut u64, s_g2_out: *mut u64) -> i32;
+    pub fn zkb_malloc(ctx: *mut zkb_ctx, bytes: u64, dptr: *mut *mut c_void) -> i32;
+    pub fn zkb_free(ctx: *mut zkb_ctx, dptr: *mut c_void) -> i32;
+    pub fn zkb_d2h(ctx: *mut zkb_ctx, dst_host: *mut c_void, src_dev: *const c_void, bytes: u64) -> i32;
     // keygen / proving key
     pub fn zkb_csf_validate(csf: *const u32, csf_words: u64) -> i32;
     pub fn zkb_keygen_pk(ctx: *mut zkb_ctx, csf: *const u32, csf_words: u64, fixed: *const *const u64, copies: *const u32, n_copies: u64,

@@ -146,7 +146,8 @@ def msm_last_adds(ctx=None):
 
 
 def g1_fixed_base_mul_dev(base_affine, scalars_t, ctx=None):
-    """out[i] = [scalars[i]] base -> torch int64 CUDA tensor (n, 8).  (ParamsKZG::unsafe_setup_with_s building block.)"""
+    """out[i] = [scalars[i]] base -> torch int64 CUDA tensor (n, 8).  Plain double-and-add: the independent
+    reference of the SRS setup tests and the source of benchmark bases."""
     import torch
     ctx = ctx or default_context(scalars_t.device.index)
     n = scalars_t.shape[0]

@@ -19,6 +19,7 @@
 //      segment partials are tree-reduced per window, and the W window sums are combined by Horner doubling.
 //   Work is dominated by n*W mixed additions = n*W*10 Fq multiplies: bound by the integer-multiply pipe.
 #include "common.cuh"
+#include "digits.cuh"
 #include <string.h>
 #include <algorithm>
 
@@ -49,14 +50,7 @@ static MsmCfg choose_cfg(uint64_t n) {
     return m;
 }
 
-// signed-digit recoding of a canonical scalar (8 x u32), window w; carry chain recomputed from window 0
-__device__ __forceinline__ uint32_t raw_window(const uint32_t s[8], uint32_t bit, uint32_t c) {
-    const uint32_t limb = bit >> 5, off = bit & 31;
-    uint64_t v = s[limb];
-    if (limb + 1 < 8) v |= (uint64_t)s[limb + 1] << 32;
-    return (uint32_t)(v >> off) & ((1u << c) - 1);
-}
-
+// signed-digit recoding of a canonical scalar (8 x u32) by signed_digit (digits.cuh); carry chain from window 0
 // mode 0: histogram; mode 1: scatter
 template <int MODE>
 __global__ void msm_digits_kernel(const Fr *const *__restrict__ scalar_cols, uint64_t n, MsmCfg m, uint32_t *__restrict__ counts,
@@ -67,11 +61,8 @@ __global__ void msm_digits_kernel(const Fr *const *__restrict__ scalar_cols, uin
     const Fr s = fp_to_canonical(fp_load(scalar_cols[blockIdx.y] + i));
     uint32_t carry = 0;
     for (uint32_t w = 0; w < m.windows; ++w) {
-        const uint32_t bit = w * m.c;
-        uint32_t d = (bit < 256 ? raw_window(s.l, bit, m.c) : 0) + carry;
-        uint32_t neg = 0;
-        if (d > m.half) { d = (1u << m.c) - d; neg = 1; carry = 1; }
-        else carry = 0;
+        uint32_t neg;
+        const uint32_t d = signed_digit(s.l, w * m.c, m.c, m.half, carry, neg);
         if (d != 0) {
             const uint32_t b = col_base + (m.shifted ? 0u : w * m.half) + (d - 1);
             if (MODE == 0) atomicAdd(&counts[b], 1u);
@@ -394,6 +385,8 @@ __global__ void __launch_bounds__(128) msm_shift_bases_kernel(const G1Affine *__
 }
 
 // ---- fixed-base scalar multiplication: out[i] = [s_i] base (affine) ------------------------------------------
+// Plain double-and-add with one inversion per point: the independent reference the SRS setup's comb (setup.cu) is tested against,
+// and the source of distinct benchmark bases.
 __global__ void __launch_bounds__(128) fixed_base_mul_kernel(G1Affine base, const Fr *__restrict__ scalars, uint64_t n, G1Affine *__restrict__ out) {
     const uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x;
     if (i >= n) return;

@@ -278,6 +278,69 @@ static uint32_t g2_sign(const Fq2 &y) {
     return c0.is_zero() ? (fp_to_canonical(y.c1).l[0] & 1u) : (c0.l[0] & 1u);
 }
 
+// ---- [s] G2 (ParamsKZG::setup's g2 / s_g2): Jacobian coordinates x = X / Z^2, y = Y / Z^3, identity Z = 0; a = 0 ----------------
+struct G2Jac { Fq2 x, y, z; };
+static Fq2 f2_sub(const Fq2 &a, const Fq2 &b) { return {fp_sub(a.c0, b.c0), fp_sub(a.c1, b.c1)}; }
+static Fq2 f2_dbl(const Fq2 &a) { return f2_add(a, a); }
+static Fq2 f2_inv(const Fq2 &a) {   // (c0 - c1 i) / (c0^2 + c1^2); 0 -> 0
+    const Fq t = fp_inv(fp_add(fp_mul(a.c0, a.c0), fp_mul(a.c1, a.c1)));
+    return {fp_mul(a.c0, t), fp_neg(fp_mul(a.c1, t))};
+}
+// the halo2curves G2 generator (canonical limbs, 8 x u32 LE per coordinate: x.c0, x.c1, y.c0, y.c1)
+static const uint32_t G2_GEN_CANON[4][8] = {
+    {0xd992f6edu, 0x46debd5cu, 0xf75edaddu, 0x674322d4u, 0x5e5c4479u, 0x426a0066u, 0x121f1e76u, 0x1800deefu},
+    {0xaef312c2u, 0x97e485b7u, 0x35a9e712u, 0xf1aa4933u, 0x31fb5d25u, 0x7260bfb7u, 0x920d483au, 0x198e9393u},
+    {0x66fa7daau, 0x4ce6cc01u, 0x0c43d37bu, 0xe3d1e769u, 0x8dcb408fu, 0x4aab7180u, 0xdb8c6debu, 0x12c85ea5u},
+    {0xd122975bu, 0x55acdadcu, 0x70b38ef3u, 0xbc4b3133u, 0x690c3395u, 0xec9e99adu, 0x585ff075u, 0x090689d0u},
+};
+static G2Jac g2_generator() {
+    Fq c[4];
+    for (int j = 0; j < 4; ++j) {
+        for (int i = 0; i < 8; ++i) c[j].l[i] = G2_GEN_CANON[j][i];
+        c[j] = fp_from_canonical(c[j]);
+    }
+    return {{c[0], c[1]}, {c[2], c[3]}, {Fq::one(), Fq::zero()}};
+}
+static G2Jac g2_identity() { return {{Fq::zero(), Fq::zero()}, {Fq::zero(), Fq::zero()}, {Fq::zero(), Fq::zero()}}; }
+static G2Jac g2_dbl(const G2Jac &p) {   // EFD dbl-2009-l
+    if (f2_is_zero(p.z)) return p;
+    const Fq2 a = f2_mul(p.x, p.x), b = f2_mul(p.y, p.y), c = f2_mul(b, b);
+    const Fq2 xb = f2_add(p.x, b);
+    const Fq2 d = f2_dbl(f2_sub(f2_sub(f2_mul(xb, xb), a), c));
+    const Fq2 e = f2_add(f2_dbl(a), a), f = f2_mul(e, e);
+    G2Jac r;
+    r.x = f2_sub(f, f2_dbl(d));
+    r.y = f2_sub(f2_mul(e, f2_sub(d, r.x)), f2_dbl(f2_dbl(f2_dbl(c))));
+    r.z = f2_dbl(f2_mul(p.y, p.z));
+    return r;
+}
+static G2Jac g2_add(const G2Jac &p, const G2Jac &q) {   // EFD add-2007-bl, complete: identity operands, doubling, inverse points
+    if (f2_is_zero(p.z)) return q;
+    if (f2_is_zero(q.z)) return p;
+    const Fq2 z1z1 = f2_mul(p.z, p.z), z2z2 = f2_mul(q.z, q.z);
+    const Fq2 u1 = f2_mul(p.x, z2z2), u2 = f2_mul(q.x, z1z1);
+    const Fq2 s1 = f2_mul(f2_mul(p.y, q.z), z2z2), s2 = f2_mul(f2_mul(q.y, p.z), z1z1);
+    const Fq2 h = f2_sub(u2, u1), rr = f2_dbl(f2_sub(s2, s1));
+    if (f2_is_zero(h)) return f2_is_zero(rr) ? g2_dbl(p) : g2_identity();
+    const Fq2 h2 = f2_dbl(h), i = f2_mul(h2, h2), j = f2_mul(h, i), v = f2_mul(u1, i);
+    G2Jac r;
+    r.x = f2_sub(f2_sub(f2_mul(rr, rr), j), f2_dbl(v));
+    r.y = f2_sub(f2_mul(rr, f2_sub(v, r.x)), f2_dbl(f2_mul(s1, j)));
+    const Fq2 zs = f2_add(p.z, q.z);
+    r.z = f2_mul(f2_sub(f2_sub(f2_mul(zs, zs), z1z1), z2z2), h);
+    return r;
+}
+static void fq_to_le_bytes(const Fq &a, uint8_t *b);
+// affine raw form (x.c0, x.c1, y.c0, y.c1, Montgomery limbs); identity = zeros
+static void g2_to_raw(const G2Jac &p, uint64_t out[16]) {
+    memset(out, 0, 16 * sizeof(uint64_t));
+    if (f2_is_zero(p.z)) return;
+    const Fq2 zi = f2_inv(p.z), zi2 = f2_mul(zi, zi), zi3 = f2_mul(zi2, zi);
+    const Fq2 x = f2_mul(p.x, zi2), y = f2_mul(p.y, zi3);
+    const Fq v[4] = {x.c0, x.c1, y.c0, y.c1};
+    for (int i = 0; i < 4; ++i) fq_to_le_bytes(v[i], (uint8_t *)out + 32 * i);
+}
+
 static Fq fq_from_le_bytes(const uint8_t *b) {
     Fq r;
     for (int i = 0; i < 8; ++i) r.l[i] = (uint32_t)b[4 * i] | (uint32_t)b[4 * i + 1] << 8 | (uint32_t)b[4 * i + 2] << 16 | (uint32_t)b[4 * i + 3] << 24;
@@ -389,6 +452,28 @@ extern "C" int32_t zkb_g2_decode_host(int32_t format, const uint8_t *in, uint64_
     if (g2_sign(y) != sign) y = f2_neg(y);
     const Fq v[4] = {x.c0, x.c1, y.c0, y.c1};
     for (int i = 0; i < 4; ++i) fq_to_le_bytes(v[i], (uint8_t *)out + 32 * i);
+    return ZKB_OK;
+}
+
+// g2_out = the G2 generator, s_g2_out = [s] g2 (double-and-add over the canonical bits of s); host only
+extern "C" int32_t zkb_g2_setup_host(const uint64_t s[4], uint64_t g2_out[16], uint64_t s_g2_out[16]) {
+    ZKB_ARG(s && g2_out && s_g2_out);
+    Fr sm;
+    memcpy(sm.l, s, 32);
+    bool below_r = false;   // the stored integer must be < r
+    for (int i = 7; i >= 0; --i) {
+        if (sm.l[i] != FrParams::P(i)) { below_r = sm.l[i] < FrParams::P(i); break; }
+    }
+    ZKB_ARG(below_r);
+    const Fr e = fp_to_canonical(sm);
+    const G2Jac g = g2_generator();
+    G2Jac acc = g2_identity();
+    for (int bit = 255; bit >= 0; --bit) {
+        acc = g2_dbl(acc);
+        if ((e.l[bit >> 5] >> (bit & 31)) & 1) acc = g2_add(acc, g);
+    }
+    g2_to_raw(g, g2_out);
+    g2_to_raw(acc, s_g2_out);
     return ZKB_OK;
 }
 

@@ -52,6 +52,8 @@ SIGNATURES = {
     "zkb_srs_commit_host": (ctypes.c_int32, [_vp, ctypes.c_int32, _vp, ctypes.c_uint64, _vp, _vp]),
     "zkb_srs_commit_batch_dev": (ctypes.c_int32, [_vp, ctypes.c_int32, _vp, ctypes.c_uint32, ctypes.c_uint64, _vp, _vp]),
     "zkb_g1_fixed_base_mul_dev": (ctypes.c_int32, [_vp, _vp, _vp, ctypes.c_uint64, _vp, _vp]),
+    "zkb_srs_setup_dev": (ctypes.c_int32, [_vp, ctypes.c_uint32, _vp, _vp, _vp, _vp]),
+    "zkb_g2_setup_host": (ctypes.c_int32, [_vp, _vp, _vp]),
     "zkb_g1_decode": (ctypes.c_int32, [_vp, ctypes.c_int32, _vp, ctypes.c_uint64, _vp, _vp, _vp]),
     "zkb_g1_encode": (ctypes.c_int32, [_vp, ctypes.c_int32, _vp, ctypes.c_uint64, _vp, _vp]),
     "zkb_g2_decode_host": (ctypes.c_int32, [ctypes.c_int32, _vp, _vp, ctypes.POINTER(ctypes.c_int32)]),

@@ -1,8 +1,9 @@
 """Host mirror of halo2_proofs::poly::kzg::commitment::ParamsKZG<Bn256> (the prover-side fields) built on the GPU.
 
-`unsafe_setup_with_s` follows ParamsKZG::unsafe_setup_with_s (used by the reference at
+`setup` / `unsafe_setup_with_s` follow ParamsKZG::setup / unsafe_setup_with_s (used by the reference at
 zkevm-circuits/src/super_circuit/test.rs:74): g[i] = [s^i] G1, g_lagrange[i] = [L_i(s)] G1 with
-L_i(s) = w^i (s^n - 1) / (n (s - w^i)).  All arithmetic runs through the CUDA kernels (no CPU field code here).
+L_i(s) = w^i (s^n - 1) / (n (s - w^i)) through zkb_srs_setup_dev, g2 and s_g2 = [s] g2 through zkb_g2_setup_host.  All field
+arithmetic runs in libzkb200 (no CPU field code here).
 """
 import ctypes
 import enum
@@ -11,7 +12,6 @@ from collections import namedtuple
 import numpy as np
 
 from . import arithmetic as A
-from . import poly
 
 
 class SerdeFormat(enum.IntEnum):
@@ -125,6 +125,28 @@ def fr_pow2k_dev(t, k):
     for _ in range(k):
         t = A.field_unop_dev(A.FR, A.UOP_SQR, t)
     return t
+
+
+def srs_setup_dev(k, s_mont, ctx=None):
+    """zkb_srs_setup_dev: s_mont (4 Montgomery limbs, stored integer < r) -> (g, g_lagrange), (2^k, 8) int64 CUDA tensors."""
+    import torch
+    from .lib import check, default_context
+    ctx = ctx or default_context()
+    n = 1 << k
+    s_h = np.ascontiguousarray(np.asarray(s_mont, dtype=np.uint64).reshape(4))
+    g = torch.empty((n, 8), dtype=torch.int64, device=f"cuda:{ctx.device}")
+    gl = torch.empty((n, 8), dtype=torch.int64, device=f"cuda:{ctx.device}")
+    check(ctx.lib.zkb_srs_setup_dev(ctx.handle, int(k), _ptr(s_h), _ptr(g), _ptr(gl), A._cur_stream()))
+    return g, gl
+
+
+def g2_setup(s_mont):
+    """zkb_g2_setup_host: -> (g2, [s] g2) as raw 128-byte points.  Host only."""
+    from .lib import check, load_library
+    s_h = np.ascontiguousarray(np.asarray(s_mont, dtype=np.uint64).reshape(4))
+    g2, s_g2 = np.zeros(16, dtype=np.uint64), np.zeros(16, dtype=np.uint64)
+    check(load_library().zkb_g2_setup_host(_ptr(s_h), _ptr(g2), _ptr(s_g2)))
+    return g2.tobytes(), s_g2.tobytes()
 
 
 def g1_generator():
@@ -243,23 +265,18 @@ class ParamsKZG:
             raise ValueError(f"Wrong params file of degree {self.k}")
 
     @staticmethod
+    def setup(k, s, ctx=None):
+        """ParamsKZG::setup / new with the caller's trapdoor s (a python int; setup's random s is drawn by the caller): g and
+        g_lagrange as (2^k, 8) device tensors (zkb_srs_setup_dev), g2 / s_g2 as raw 128-byte points (zkb_g2_setup_host).  When
+        s^n = 1 g_lagrange is the true Lagrange basis (see include/zkb200.h), where upstream panics."""
+        s_mont = fr_scalar_dev(s).cpu().numpy().view(np.uint64)[0].copy()
+        g, gl = srs_setup_dev(k, s_mont, ctx=ctx)
+        g2, s_g2 = g2_setup(s_mont)
+        return ParamsKZG(k, g, gl, g2, s_g2)
+
+    @staticmethod
     def unsafe_setup_with_s(k, s):
-        n = 1 << k
-        gen = g1_generator()
-        s_t = fr_scalar_dev(s)
-        s_host = s_t.cpu().numpy().view(np.uint64)[0]
-        pw = poly.fr_powers_dev(s_host, n)
-        g = A.g1_fixed_base_mul_dev(gen, pw)
-        omega, _ = A.root_of_unity(k)
-        W = poly.fr_powers_dev(omega, n)
-        den = A.field_binop_dev(A.FR, A.OP_SUB, bcast(s_t, n), W)
-        inv = A.fr_batch_invert_dev(den)
-        one = fr_scalar_dev(1)
-        c1 = A.field_binop_dev(A.FR, A.OP_MUL, A.field_binop_dev(A.FR, A.OP_SUB, fr_pow2k_dev(s_t, k), one),
-                               A.field_unop_dev(A.FR, A.UOP_INV, fr_scalar_dev(n)))
-        L = A.field_binop_dev(A.FR, A.OP_MUL, A.field_binop_dev(A.FR, A.OP_MUL, W, inv), bcast(c1, n))
-        gl = A.g1_fixed_base_mul_dev(gen, L)
-        return ParamsKZG(k, g, gl)
+        return ParamsKZG.setup(k, s)
 
     def commit_lagrange(self, values_dev):
         return A.best_multiexp_dev(values_dev, self.g_lagrange)
