@@ -1,9 +1,10 @@
 """Model of the configuration choices and the work accounting of csrc/msm.cu, in vectorised numpy: the window size
-(`choose_cfg`), the shifted-SRS window size and copy count, the per-pass batch limit, the signed-digit recoding of
-`msm_digits_kernel` (32-bit limbs, carry chain from window 0), the bucket index of a digit, the scratch bounds of
-`msm_g1_batch_device_ex`, and what `zkb_msm_last_adds` / `zkb_msm_last_levels` report after an MSM.  Names follow the
-kernel.  tests/test_msm_model.py checks it on the CPU; the GPU tests compare the library's counters with it, which proves
-which configuration an MSM ran.  It is a check of the host logic and the accounting -- not a product path."""
+(`msm_cfg`, whose plain branch is `choose_cfg`), the shifted-SRS window size and copy count, the per-pass batch limit, the
+signed-digit recoding of `msm_digits_kernel` (32-bit limbs, carry chain from window 0), the bucket index of a digit, the
+scratch bounds and argument checks of `msm_plan`, and what `zkb_msm_last_adds` / `zkb_msm_last_levels` report after an
+MSM.  Names follow the kernel.  tests/test_msm_model.py checks it on the CPU; the GPU tests compare the library's counters
+with it, which proves which configuration an MSM ran.  It is a check of the host logic and the accounting -- not a product
+path."""
 import numpy as np
 
 R_MOD = 0x30644E72E131A029B85045B68181585D2833E84879B9709143E1F593F0000001
@@ -54,7 +55,7 @@ def msm_max_batch(n):
 
 
 def msm_cfg(n, shifted):
-    """the configuration msm_g1_batch_device_ex runs for n points (shifted: against msm_shift_copies(n) copies of the bases)"""
+    """the configuration a pass runs for n points (shifted: against msm_shift_copies(n) copies of the bases)"""
     if not shifted:
         return choose_cfg(n)
     c = msm_shift_window_bits(n)
@@ -140,7 +141,7 @@ def level0_partials(counts):
 
 
 def level_bound(n, cfg):
-    """msm_g1_batch_device_ex's bound: partials of the fullest possible bucket (n entries, n * W when shifted), and the
+    """msm_plan's bound: partials of the fullest possible bucket (n entries, n * W when shifted), and the
     number of reduction levels it launches for it"""
     bound = (n * (cfg.windows if cfg.shifted else 1) + CHUNK - 1) // CHUNK + 1
     b, launched = bound, 0
@@ -174,7 +175,7 @@ def predict(col_counts, n, cfg):
     return int(counts.sum()) + extra + 2 * counts.size, run
 
 
-# ---- scratch bounds and argument limits of msm_g1_batch_device_ex ------------------------------------------------------
+# ---- scratch bounds and argument limits of msm_plan ------------------------------------------------------------------
 def scratch(n, batch, shifted):
     cfg = msm_cfg(n, shifted)
     rwin1 = 1 if shifted else cfg.windows
@@ -187,7 +188,7 @@ def scratch(n, batch, shifted):
 
 
 def arg_failures(n, batch, shifted):
-    """the ZKB_ARG checks of msm_g1_batch_device_ex that would refuse this call (empty: it runs)"""
+    """the ZKB_ARG checks of msm_plan that would refuse this call (empty: it runs)"""
     sc = scratch(n, batch, shifted)
     cfg, bad = sc["cfg"], []
     if not n < (1 << 31):

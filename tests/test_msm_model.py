@@ -48,7 +48,7 @@ def sizes_up_to_2_28():
 
 
 def test_argument_limits():
-    """For every n <= 2^28 (the largest SRS) and every batch up to msm_max_batch(n), none of msm_g1_batch_device_ex's
+    """For every n <= 2^28 (the largest SRS) and every batch up to msm_max_batch(n), none of msm_plan's
     argument checks refuses the call, plain or against shifted copies.  Catches a batch limit that lets a pass overflow
     the 32-bit pair list or bucket index.  (A plain MSM of more than 2^32 / 13 points is refused: pairs >= 2^32.)"""
     for n in sizes_up_to_2_28():
@@ -94,7 +94,7 @@ def straddling_counts(sc, n):
 @pytest.mark.parametrize("shifted", [False, True])
 def test_worst_case_scratch(shifted):
     """The level-0 partials, the outputs of every later level (written alternately to part[1] and part[0]) and the number of
-    levels stay within what msm_g1_batch_device_ex allocates from its bounds, for all scalars in one bucket and for every
+    levels stay within what msm_plan allocates from its bounds, for all scalars in one bucket and for every
     bucket straddling chunk boundaries, at every size 2^3 ... 2^28 with one column and with msm_max_batch columns.
     Catches a partial buffer sized without the one-extra-partial-per-bucket term, or a missing reduction level."""
     for lg in range(3, 29):

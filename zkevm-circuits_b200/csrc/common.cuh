@@ -160,17 +160,19 @@ struct NttPeerRoute {
 };
 int32_t ntt_fr_batch_device_ex(zkb_ctx *ctx, const Fr *const *h_src, Fr *const *h_dst, uint32_t count, uint32_t log_n, const Fr &omega,
                                const Fr *scale_host, int coset_zeta, const Fr *d_in_scale, const NttPeerRoute *route, cudaStream_t st);
-// synchronises: the result point is returned to the host
+// MSMs synchronise: their results are returned to the host
 int32_t msm_g1_device(zkb_ctx *ctx, const Fr *scalars, const G1Affine *bases, uint64_t n, G1Affine *out_affine_host, cudaStream_t st);
-// `batch` MSMs over the same bases in one pass (d_scalar_cols: DEVICE array of device pointers; batch <= msm_max_batch(n))
+// `count` MSMs over the same bases (h_cols: HOST array of device pointers), in passes of msm_max_batch(n) columns.  shifted: `bases`
+// holds the msm_shift_copies(n) x n points of msm_build_shifted_bases
+int32_t msm_g1_columns(zkb_ctx *ctx, const Fr *const *h_cols, uint32_t count, const G1Affine *bases, uint64_t n, G1Affine *out_host,
+                       bool shifted, cudaStream_t st);
+// columns per pass: bounded by the 32-bit pair list and, against shifted bases, by the size of the bucket arrays
 uint32_t msm_max_batch(uint64_t n);
 // window-shifted precomputed bases (copy w = 2^(c w) P_i): one bucket set per column, no Horner
 uint32_t msm_shift_copies(uint64_t n);
 int32_t msm_build_shifted_bases(zkb_ctx *ctx, const G1Affine *bases, uint64_t n, G1Affine *out, cudaStream_t st);
-int32_t msm_g1_batch_device_ex(zkb_ctx *ctx, const Fr *const *d_scalar_cols, uint32_t batch, const G1Affine *bases, uint64_t n,
-                               G1Affine *out_affine_host, bool shifted, cudaStream_t st);
-int32_t msm_g1_batch_device(zkb_ctx *ctx, const Fr *const *d_scalar_cols, uint32_t batch, const G1Affine *bases, uint64_t n,
-                            G1Affine *out_affine_host, cudaStream_t st);
+// the ABI's outputs of a G1 result: affine limbs, and Jacobian limbs (z = 1, or 0 for the identity) / compressed bytes where not null
+void g1_emit(const G1Affine &r, uint64_t out_affine[8], uint64_t *out_jacobian, uint8_t *out_compressed);
 // SRS handle (srs.cu): sources on the host or on the device; g_lagrange == nullptr -> derived on the device (g_to_lagrange)
 int32_t srs_create(zkb_ctx *ctx, uint32_t k, const G1Affine *g, bool g_on_device, const G1Affine *g_lagrange, bool gl_on_device, zkb_srs **out);
 // `count` commitments against basis 0 (g) / 1 (g_lagrange); cols = HOST array of device pointers; synchronises (results on the host)

@@ -29,26 +29,9 @@ struct MsmCfg {
     uint32_t c;         // window bits
     uint32_t windows;   // W
     uint32_t half;      // 2^(c-1) buckets per window
-    uint32_t seg_log;   // unused
     uint32_t shifted;   // 1: bases array holds W copies, copy w = 2^(c w) * P_i -> ONE bucket set per column, no Horner
     uint32_t n32;       // points per copy (shifted mode)
 };
-
-static MsmCfg choose_cfg(uint64_t n) {
-    uint32_t lg = 0;
-    while ((1ull << (lg + 1)) <= n) ++lg;
-    int c = (int)lg - 4;
-    if (c < 3) c = 3;
-    if (c > 20) c = 20;
-    MsmCfg m;
-    m.c = (uint32_t)c;
-    m.windows = (255 + m.c - 1) / m.c;
-    m.half = 1u << (m.c - 1);
-    m.seg_log = 0;
-    m.shifted = 0;
-    m.n32 = 0;
-    return m;
-}
 
 // signed-digit recoding of a canonical scalar (8 x u32) by signed_digit (digits.cuh); carry chain from window 0
 // mode 0: histogram; mode 1: scatter
@@ -102,7 +85,14 @@ __device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t *t
     return base + x - v;
 }
 
-__global__ void scan_blocks_kernel(const uint32_t *__restrict__ in, uint32_t *__restrict__ out, uint32_t *__restrict__ block_sums, uint64_t n) {
+// GATED: the scans of the bucket accumulation's levels >= 1.  They do nothing unless the device-side MsmState says a level is
+// needed (st_words[0] = maxlen > 1), and write toff[cur ^ 1] (st_words[1] = cur: out0 when cur == 1, out1 when cur == 0).
+// Plain: out0.
+template <bool GATED>
+__global__ void scan_blocks_kernel(const uint32_t *__restrict__ in, uint32_t *const out0, uint32_t *const out1, const uint32_t *st_words,
+                                   uint32_t *__restrict__ block_sums, uint64_t n) {
+    if (GATED && st_words[0] <= 1) return;
+    uint32_t *out = GATED ? (st_words[1] ? out0 : out1) : out0;
     __shared__ uint32_t sm[32];
     const uint64_t base = (uint64_t)blockIdx.x * SCAN_BLK + (uint64_t)threadIdx.x * SCAN_PER;
     uint32_t v[SCAN_PER], sum = 0;
@@ -114,50 +104,12 @@ __global__ void scan_blocks_kernel(const uint32_t *__restrict__ in, uint32_t *__
     for (int k = 0; k < SCAN_PER; ++k) { if (base + k < n) out[base + k] = ex; ex += v[k]; }
     if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
 }
-__global__ void scan_sums_kernel(uint32_t *__restrict__ block_sums, uint32_t nblocks, uint32_t *__restrict__ grand_total) {
+template <bool GATED>
+__global__ void scan_sums_kernel(uint32_t *__restrict__ block_sums, uint32_t nblocks, uint32_t *const out0, uint32_t *const out1,
+                                 const uint32_t *st_words, uint64_t n) {
     // single block; serial over chunks of SCAN_T
-    __shared__ uint32_t sm[32];
-    uint32_t running = 0;
-    for (uint32_t s = 0; s < nblocks; s += SCAN_T) {
-        const uint32_t idx = s + threadIdx.x;
-        const uint32_t v = idx < nblocks ? block_sums[idx] : 0;
-        uint32_t total;
-        const uint32_t ex = block_exclusive_scan(v, &total, sm);
-        if (idx < nblocks) block_sums[idx] = running + ex;
-        running += total;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0 && grand_total) *grand_total = running;
-}
-__global__ void scan_add_kernel(uint32_t *__restrict__ out, const uint32_t *__restrict__ block_sums, uint64_t n) {
-    const uint64_t base = (uint64_t)blockIdx.x * SCAN_BLK + (uint64_t)threadIdx.x * SCAN_PER;
-    const uint32_t add = block_sums[blockIdx.x];
-#pragma unroll
-    for (int k = 0; k < SCAN_PER; ++k)
-        if (base + k < n) out[base + k] += add;
-}
-
-// the same three kernels for the gated reduction levels: the scan of tcount goes to toff[cur ^ 1]
-struct MsmState;
-__global__ void scan_blocks_gated_kernel(const uint32_t *__restrict__ in, uint32_t *const outs0, uint32_t *const outs1, const uint32_t *st_words,
-                                         uint32_t *__restrict__ block_sums, uint64_t n) {
-    if (st_words[0] <= 1) return;   // MsmState::maxlen
-    uint32_t *out = st_words[1] ? outs0 : outs1;   // cur == 1 -> write toff[0]
-    __shared__ uint32_t sm[32];
-    const uint64_t base = (uint64_t)blockIdx.x * SCAN_BLK + (uint64_t)threadIdx.x * SCAN_PER;
-    uint32_t v[SCAN_PER], sum = 0;
-#pragma unroll
-    for (int k = 0; k < SCAN_PER; ++k) { v[k] = base + k < n ? in[base + k] : 0; sum += v[k]; }
-    uint32_t total;
-    uint32_t ex = block_exclusive_scan(sum, &total, sm);
-#pragma unroll
-    for (int k = 0; k < SCAN_PER; ++k) { if (base + k < n) out[base + k] = ex; ex += v[k]; }
-    if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
-}
-__global__ void scan_sums_gated_kernel(uint32_t *__restrict__ block_sums, uint32_t nblocks, uint32_t *const outs0, uint32_t *const outs1,
-                                       const uint32_t *st_words, uint64_t n) {
-    if (st_words[0] <= 1) return;
-    uint32_t *out = st_words[1] ? outs0 : outs1;
+    if (GATED && st_words[0] <= 1) return;
+    uint32_t *out = GATED ? (st_words[1] ? out0 : out1) : out0;
     __shared__ uint32_t sm[32];
     uint32_t running = 0;
     for (uint32_t s = 0; s < nblocks; s += SCAN_T) {
@@ -171,10 +123,11 @@ __global__ void scan_sums_gated_kernel(uint32_t *__restrict__ block_sums, uint32
     }
     if (threadIdx.x == 0) out[n] = running;
 }
-__global__ void scan_add_gated_kernel(uint32_t *const outs0, uint32_t *const outs1, const uint32_t *st_words, const uint32_t *__restrict__ block_sums,
-                                      uint64_t n) {
-    if (st_words[0] <= 1) return;
-    uint32_t *out = st_words[1] ? outs0 : outs1;
+template <bool GATED>
+__global__ void scan_add_kernel(uint32_t *const out0, uint32_t *const out1, const uint32_t *st_words, const uint32_t *__restrict__ block_sums,
+                                uint64_t n) {
+    if (GATED && st_words[0] <= 1) return;
+    uint32_t *out = GATED ? (st_words[1] ? out0 : out1) : out0;
     const uint64_t base = (uint64_t)blockIdx.x * SCAN_BLK + (uint64_t)threadIdx.x * SCAN_PER;
     const uint32_t add = block_sums[blockIdx.x];
 #pragma unroll
@@ -182,12 +135,14 @@ __global__ void scan_add_gated_kernel(uint32_t *const outs0, uint32_t *const out
         if (base + k < n) out[base + k] += add;
 }
 
-// out[0..n) = exclusive scan of in, out[n] = total.  tmp: ceil(n / SCAN_BLK) u32
-static void exclusive_scan_u32(zkb_ctx *ctx, const uint32_t *in, uint32_t *out, uint64_t n, uint32_t *tmp, cudaStream_t st) {
+// out[0..n) = exclusive scan of in, out[n] = total (out = out0 unless GATED, see above).  tmp: ceil(n / SCAN_BLK) u32
+template <bool GATED>
+static void exclusive_scan_u32(zkb_ctx *ctx, const uint32_t *in, uint32_t *out0, uint32_t *out1, const uint32_t *st_words, uint64_t n,
+                               uint32_t *tmp, cudaStream_t st) {
     const uint32_t nblocks = (uint32_t)((n + SCAN_BLK - 1) / SCAN_BLK);
-    scan_blocks_kernel<<<nblocks, SCAN_T, 0, st>>>(in, out, tmp, n);
-    scan_sums_kernel<<<1, SCAN_T, 0, st>>>(tmp, nblocks, out + n);
-    scan_add_kernel<<<nblocks, SCAN_T, 0, st>>>(out, tmp, n);
+    scan_blocks_kernel<GATED><<<nblocks, SCAN_T, 0, st>>>(in, out0, out1, st_words, tmp, n);
+    scan_sums_kernel<GATED><<<1, SCAN_T, 0, st>>>(tmp, nblocks, out0, out1, st_words, n);
+    scan_add_kernel<GATED><<<nblocks, SCAN_T, 0, st>>>(out0, out1, st_words, tmp, n);
     ctx->launches += 3;
 }
 
@@ -400,27 +355,15 @@ __global__ void __launch_bounds__(128) fixed_base_mul_kernel(G1Affine base, cons
 }
 
 static size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-
-uint32_t msm_shift_window_bits(uint64_t n);
-uint32_t msm_max_batch(uint64_t n) {
-    if (n == 0) return 64;
-    const MsmCfg m = choose_cfg(n);
-    uint64_t b = (1ull << 28) / (n * m.windows);
-    const uint32_t cs = msm_shift_window_bits(n);
-    if (cs) {  // shifted mode: half * batch buckets of 128 B (+ partials): keep the bucket arrays under ~2 GiB
-        const uint64_t bb = (1ull << 31) / ((1ull << (cs - 1)) * 3 * sizeof(G1Xyzz));
-        if (bb < b) b = bb;
-    }
-    if (b < 1) b = 1;
-    if (b > 64) b = 64;
-    return (uint32_t)b;
-}
-
-// batch of `batch` MSMs over the same bases: d_scalar_cols is a DEVICE array of `batch` device pointers
-// window bits used with precomputed shifted bases for n points (0 = not supported at this size)
-uint32_t msm_shift_window_bits(uint64_t n) {
+static uint32_t log2_floor(uint64_t n) {
     uint32_t lg = 0;
     while ((1ull << (lg + 1)) <= n) ++lg;
+    return lg;
+}
+
+// window bits used with precomputed shifted bases for n points (0 = not supported at this size)
+uint32_t msm_shift_window_bits(uint64_t n) {
+    const uint32_t lg = log2_floor(n);
     if (lg < 10 || lg > 22) return 0;
     return lg > 20 ? 20 : lg;
 }
@@ -441,178 +384,245 @@ int32_t msm_build_shifted_bases(zkb_ctx *ctx, const G1Affine *bases, uint64_t n,
     return ZKB_OK;
 }
 
-int32_t msm_g1_batch_device_ex(zkb_ctx *ctx, const Fr *const *d_scalar_cols, uint32_t batch, const G1Affine *bases, uint64_t n,
-                               G1Affine *out_affine_host, bool shifted, cudaStream_t st);
-
-int32_t msm_g1_batch_device(zkb_ctx *ctx, const Fr *const *d_scalar_cols, uint32_t batch, const G1Affine *bases, uint64_t n,
-                            G1Affine *out_affine_host, cudaStream_t st) {
-    return msm_g1_batch_device_ex(ctx, d_scalar_cols, batch, bases, n, out_affine_host, false, st);
-}
-
-// shifted == true: `bases` holds msm_shift_copies(n) x n points built by msm_build_shifted_bases
-int32_t msm_g1_batch_device_ex(zkb_ctx *ctx, const Fr *const *d_scalar_cols, uint32_t batch, const G1Affine *bases, uint64_t n,
-                               G1Affine *out_affine_host, bool shifted, cudaStream_t st) {
-    ZKB_ARG(n < (1ull << 31) && batch >= 1);
-    if (n == 0) {
-        memset(out_affine_host, 0, sizeof(G1Affine) * batch);
-        ctx->msm_last_adds = 0;
-        return ZKB_OK;
-    }
-    MsmCfg m = choose_cfg(n);
-    if (shifted) {
-        m.c = msm_shift_window_bits(n);
-        ZKB_ARG(m.c != 0);
+// window configuration for n points: c = log2(n) - 4 within [3, 20]; against shifted bases c = msm_shift_window_bits(n), which is
+// 0 where no copies exist
+static MsmCfg msm_cfg(uint64_t n, bool shifted) {
+    MsmCfg m = {};
+    m.c = shifted ? msm_shift_window_bits(n) : (uint32_t)std::clamp((int)log2_floor(n) - 4, 3, 20);
+    if (m.c) {
         m.windows = (255 + m.c - 1) / m.c;
         m.half = 1u << (m.c - 1);
-        m.shifted = 1;
-        m.n32 = (uint32_t)n;
-        ZKB_ARG((uint64_t)m.windows * n < (1ull << 31));
     }
-    const uint32_t windows1 = m.windows;          // digit windows per column
-    const uint32_t rwin1 = shifted ? 1 : windows1;  // bucket sets (reduction windows) per column
-    const uint32_t nbuckets = batch * rwin1 * m.half;
-    const uint64_t pairs = n * windows1 * batch;
-    ZKB_ARG(pairs < (1ull << 32) && (uint64_t)batch * rwin1 * m.half < (1ull << 31));
-    // window-reduction segment length 2^log_l: short segments when a single column would otherwise leave the SMs empty
-    uint32_t log_l = 5;
-    while (log_l > 3 && (uint64_t)batch * rwin1 * (m.half >> log_l) < 32768) --log_l;
+    m.shifted = shifted;
+    m.n32 = shifted ? (uint32_t)n : 0;
+    return m;
+}
 
-    // scratch A: counts | offsets(+1) | cursors | tcount | toffA(+1) | toffB(+1) | scan tmp | state
-    const size_t cnt_bytes = align_up((size_t)(nbuckets + 2) * 4, 256);
-    const size_t tmp_bytes = align_up(((size_t)nbuckets / SCAN_BLK + 2) * 4, 256);
+uint32_t msm_max_batch(uint64_t n) {
+    if (n == 0) return 64;
+    uint64_t b = (1ull << 28) / (n * msm_cfg(n, false).windows);
+    const MsmCfg s = msm_cfg(n, true);
+    if (s.c) {  // shifted mode: half * batch buckets of 128 B (+ partials): keep the bucket arrays under ~2 GiB
+        const uint64_t bb = (1ull << 31) / ((uint64_t)s.half * 3 * sizeof(G1Xyzz));
+        if (bb < b) b = bb;
+    }
+    return (uint32_t)std::clamp<uint64_t>(b, 1, 64);
+}
+
+// ---- one pass: `batch` MSMs over the same bases --------------------------------------------------------------------------
+// Everything a pass allocates is sized on the host from bounds, so no count returns from the device before the result does.
+// tests/msm_model.py (msm_cfg, msm_max_batch, level_bound, scratch, arg_failures) restates these numbers.
+struct MsmPlan {
+    MsmCfg m;
+    uint64_t n, pairs;     // pairs: (point, window) pairs of the pass
+    uint32_t batch;
+    uint32_t sets;         // bucket sets (reduction windows) per column: 1 against shifted bases, W otherwise
+    uint32_t wred;         // reduction windows of the pass: sets x batch
+    uint32_t nbuckets;     // wred x half
+    uint32_t acc_levels;   // gated accumulation levels >= 1: enough for the partials of the fullest possible bucket
+    uint32_t log_l;        // window reduction: segments of 2^log_l buckets ...
+    uint32_t nlevels;      // ... reduced in this many levels
+    size_t level_entries;  // G1Xyzz written by the window-reduction levels (acc and run outputs)
+    size_t part0_n;        // bound of the level-0 partials: one per chunk plus one per bucket
+    size_t part1_n;        // bound of every later level's partials: previous / ACC_CH plus one per bucket
+    // scratch A, bytes: counts | offsets (+1) | cursors | tcount | toff[0] (+1) | toff[1] (+1), at k * cnt_bytes, then the
+    // scan tmp at a_scan_tmp and the MsmState at a_state
+    size_t cnt_bytes, a_scan_tmp, a_state, a_bytes;
+    size_t b_bytes;        // scratch B: the sorted pair list, 4 B per pair
+    // scratch C, bytes: part[0] at 0 | part[1] | buckets | window-reduction levels | level sums | all-bucket sums | window results
+    size_t c_part1, c_buckets, c_lvl, c_lvl_sums, c_all_sum, c_wres, c_bytes;
+};
+
+// shifted: against msm_shift_copies(n) x n bases built by msm_build_shifted_bases.  Refuses what the 32-bit pair list and bucket
+// indices cannot hold.
+static int32_t msm_plan(uint64_t n, uint32_t batch, bool shifted, MsmPlan *out) {
+    ZKB_ARG(n < (1ull << 31) && batch >= 1);
+    MsmPlan p = {};
+    p.m = msm_cfg(n, shifted);
+    ZKB_ARG(p.m.c != 0);
+    ZKB_ARG(!shifted || (uint64_t)p.m.windows * n < (1ull << 31));
+    p.n = n;
+    p.batch = batch;
+    p.sets = shifted ? 1 : p.m.windows;
+    p.pairs = n * p.m.windows * batch;
+    ZKB_ARG(p.pairs < (1ull << 32) && (uint64_t)batch * p.sets * p.m.half < (1ull << 31));
+    p.wred = p.sets * batch;
+    p.nbuckets = p.wred * p.m.half;
+    for (uint64_t bound = (n * (shifted ? p.m.windows : 1) + CHUNK - 1) / CHUNK + 1; bound > 1; bound = (bound + ACC_CH - 1) / ACC_CH)
+        p.acc_levels++;
+    // short window-reduction segments when a single column would otherwise leave the SMs empty; c >= 3, so at least one level
+    p.log_l = 5;
+    while (p.log_l > 3 && (uint64_t)p.wred * (p.m.half >> p.log_l) < 32768) --p.log_l;
+    for (uint32_t cnt = p.m.half; cnt > 1; p.nlevels++) {
+        cnt = (cnt + (1u << p.log_l) - 1) >> p.log_l;
+        p.level_entries += 2ull * cnt * p.wred;
+    }
+    p.part0_n = (size_t)((p.pairs + CHUNK - 1) / CHUNK) + p.nbuckets + 1;
+    p.part1_n = p.part0_n / ACC_CH + p.nbuckets + 1;
+    ZKB_ARG(p.part0_n < (1ull << 32));
+
+    p.cnt_bytes = align_up((size_t)(p.nbuckets + 2) * 4, 256);
+    p.a_scan_tmp = 6 * p.cnt_bytes;
+    p.a_state = p.a_scan_tmp + align_up(((size_t)p.nbuckets / SCAN_BLK + 2) * 4, 256);
+    p.a_bytes = p.a_state + 256;
+    p.b_bytes = p.pairs * 4;
+    p.c_part1 = p.part0_n * sizeof(G1Xyzz);
+    p.c_buckets = p.c_part1 + p.part1_n * sizeof(G1Xyzz);
+    p.c_lvl = p.c_buckets + (size_t)p.nbuckets * sizeof(G1Xyzz);
+    p.c_lvl_sums = p.c_lvl + p.level_entries * sizeof(G1Xyzz);
+    p.c_all_sum = p.c_lvl_sums + (size_t)p.nlevels * p.wred * sizeof(G1Xyzz);
+    p.c_wres = p.c_all_sum + (size_t)p.wred * sizeof(G1Xyzz);
+    p.c_bytes = p.c_wres + (size_t)p.wred * sizeof(G1Xyzz);
+    *out = p;
+    return ZKB_OK;
+}
+
+// the plan's arrays in the context's scratch arenas
+struct MsmBufs {
+    uint32_t *counts, *offsets, *cursors, *tcount, *toff[2], *scan_tmp, *sorted;
+    MsmState *state;
+    G1Xyzz *part[2], *buckets, *lvl, *lvl_sums, *all_sum, *wres;
+};
+static int32_t msm_scratch(zkb_ctx *ctx, const MsmPlan &p, MsmBufs *b) {
     uint8_t *A = nullptr, *B = nullptr, *C = nullptr;
-    ZKB_TRY(scratch_get(ctx, SCR_MSM_A, 6 * cnt_bytes + tmp_bytes + 256, (void **)&A));
-    ZKB_TRY(scratch_get(ctx, SCR_MSM_B, pairs * 4, (void **)&B));
-    uint32_t *counts = (uint32_t *)A, *offsets = (uint32_t *)(A + cnt_bytes), *cursors = (uint32_t *)(A + 2 * cnt_bytes);
-    uint32_t *tcount = (uint32_t *)(A + 3 * cnt_bytes), *toff[2] = {(uint32_t *)(A + 4 * cnt_bytes), (uint32_t *)(A + 5 * cnt_bytes)};
-    uint32_t *scan_tmp = (uint32_t *)(A + 6 * cnt_bytes);
-    MsmState *d_state = (MsmState *)(A + 6 * cnt_bytes + tmp_bytes);
-    uint32_t *sorted = (uint32_t *)B;
+    ZKB_TRY(scratch_get(ctx, SCR_MSM_A, p.a_bytes, (void **)&A));
+    ZKB_TRY(scratch_get(ctx, SCR_MSM_B, p.b_bytes, (void **)&B));
+    ZKB_TRY(scratch_get(ctx, SCR_MSM_C, p.c_bytes, (void **)&C));
+    auto a = [&](int k) { return (uint32_t *)(A + k * p.cnt_bytes); };
+    auto c = [&](size_t off) { return (G1Xyzz *)(C + off); };
+    b->counts = a(0), b->offsets = a(1), b->cursors = a(2), b->tcount = a(3), b->toff[0] = a(4), b->toff[1] = a(5);
+    b->scan_tmp = (uint32_t *)(A + p.a_scan_tmp);
+    b->state = (MsmState *)(A + p.a_state);
+    b->sorted = (uint32_t *)B;
+    b->part[0] = c(0), b->part[1] = c(p.c_part1), b->buckets = c(p.c_buckets), b->lvl = c(p.c_lvl), b->lvl_sums = c(p.c_lvl_sums);
+    b->all_sum = c(p.c_all_sum), b->wres = c(p.c_wres);
+    return ZKB_OK;
+}
 
-    // scratch C, sized from BOUNDS (no count returns to the host): level 0 emits at most one partial per chunk plus one per
-    // bucket; every later level at most (previous / ACC_CH + one per bucket)
-    const uint32_t half = m.half;
-    const uint32_t wred = rwin1 * batch;  // reduction windows: from the scatter on a (column, bucket set) pair is just a window
-    uint32_t nlevels = 0, cnt = half;
-    size_t level_entries = 0;
-    while (cnt > 1) { cnt = (cnt + (1u << log_l) - 1) >> log_l; level_entries += 2ull * cnt * wred; nlevels++; }
-    if (nlevels == 0) { nlevels = 1; level_entries = 2ull * wred; }  // half == 1: one trivial level
-    const size_t part0_n = (size_t)((pairs + CHUNK - 1) / CHUNK) + nbuckets + 1;
-    const size_t part1_n = part0_n / ACC_CH + nbuckets + 1;
-    ZKB_ARG(part0_n < (1ull << 32));
-    const size_t c_entries = part0_n + part1_n + nbuckets + level_entries + (size_t)nlevels * wred + 2ull * wred;
-    ZKB_TRY(scratch_get(ctx, SCR_MSM_C, c_entries * sizeof(G1Xyzz), (void **)&C));
-    G1Xyzz *part[2] = {(G1Xyzz *)C, (G1Xyzz *)C + part0_n};
-    G1Xyzz *buckets = part[1] + part1_n, *lvl = buckets + nbuckets, *lvl_sums = lvl + level_entries, *all_sum = lvl_sums + (size_t)nlevels * wred,
-           *wres = all_sum + wred;
+// counting sort of the (point, window) pairs by bucket: histogram, scan, scatter
+static int32_t msm_sort(zkb_ctx *ctx, const MsmPlan &p, const MsmBufs &b, const Fr *const *d_cols, cudaStream_t st) {
+    ZKB_CUDA(cudaMemsetAsync(b.counts, 0, p.cnt_bytes, st));
+    const dim3 grid((unsigned)((p.n + 255) / 256), p.batch);
+    msm_digits_kernel<0><<<grid, 256, 0, st>>>(d_cols, p.n, p.m, b.counts, nullptr, nullptr);
+    exclusive_scan_u32<false>(ctx, b.counts, b.offsets, nullptr, nullptr, p.nbuckets, b.scan_tmp, st);
+    ZKB_CUDA(cudaMemcpyAsync(b.cursors, b.offsets, (size_t)p.nbuckets * 4, cudaMemcpyDeviceToDevice, st));
+    msm_digits_kernel<1><<<grid, 256, 0, st>>>(d_cols, p.n, p.m, nullptr, b.cursors, b.sorted);
+    ctx->launches += 2;
+    return ZKB_OK;
+}
 
-    ZKB_CUDA(cudaMemsetAsync(counts, 0, cnt_bytes, st));
-    ZKB_CUDA(cudaMemsetAsync(d_state, 0, sizeof(MsmState), st));
-    const unsigned tb = 256, bb = (nbuckets + 255) / 256;
-    const dim3 gb((unsigned)((n + tb - 1) / tb), batch);
-    msm_digits_kernel<0><<<gb, tb, 0, st>>>(d_scalar_cols, n, m, counts, nullptr, nullptr);
-    exclusive_scan_u32(ctx, counts, offsets, nbuckets, scan_tmp, st);
-    ZKB_CUDA(cudaMemcpyAsync(cursors, offsets, (size_t)nbuckets * 4, cudaMemcpyDeviceToDevice, st));
-    msm_digits_kernel<1><<<gb, tb, 0, st>>>(d_scalar_cols, n, m, nullptr, cursors, sorted);
-    m.windows = wred;
-    chunk_count_kernel<<<bb, 256, 0, st>>>(offsets, nbuckets, tcount, d_state);
-    exclusive_scan_u32(ctx, tcount, toff[0], nbuckets, scan_tmp, st);
-    // level 0: one thread per 32-entry chunk of the sorted list (grid from the bound; surplus threads exit on the device-side total)
-    {
-        const uint64_t max_chunks = (pairs + CHUNK - 1) / CHUNK;
+// bucket accumulation: level 0 over the 32-entry chunks of the sorted list, the gated levels >= 1, then one value per bucket
+static int32_t msm_accumulate(zkb_ctx *ctx, const MsmPlan &p, const MsmBufs &b, const G1Affine *bases, cudaStream_t st) {
+    ZKB_CUDA(cudaMemsetAsync(b.state, 0, sizeof(MsmState), st));
+    const unsigned bb = (p.nbuckets + 255) / 256;
+    chunk_count_kernel<<<bb, 256, 0, st>>>(b.offsets, p.nbuckets, b.tcount, b.state);
+    exclusive_scan_u32<false>(ctx, b.tcount, b.toff[0], nullptr, nullptr, p.nbuckets, b.scan_tmp, st);
+    {   // one thread per chunk (grid from the bound; surplus threads exit on the device-side total)
+        const uint64_t max_chunks = (p.pairs + CHUNK - 1) / CHUNK;
         ProfScope ps_(ctx, PROF_MSM_ACC, st);
-        msm_acc_chunk_kernel<<<(unsigned)((max_chunks + 127) / 128), 128, 0, st>>>(bases, offsets, sorted, toff[0], nbuckets, part[0]);
+        msm_acc_chunk_kernel<<<(unsigned)((max_chunks + 127) / 128), 128, 0, st>>>(bases, b.offsets, b.sorted, b.toff[0], p.nbuckets, b.part[0]);
     }
-    ctx->launches += 4;
-    // levels >= 1: as many as the longest possible partial list needs; each one exits at once when the lists are already single
-    LevelBufs L;
-    L.toff[0] = toff[0]; L.toff[1] = toff[1];
-    L.part[0] = part[0]; L.part[1] = part[1];
-    L.tcount = tcount;
-    L.st = d_state;
-    {
-        uint64_t bound = (n * (shifted ? windows1 : 1) + CHUNK - 1) / CHUNK + 1;   // partials of the fullest possible bucket
-        const uint32_t nscan = (uint32_t)(((uint64_t)nbuckets + SCAN_BLK - 1) / SCAN_BLK);
-        const uint32_t *stw = (const uint32_t *)d_state;
-        const unsigned lv_blocks = (unsigned)std::min<uint64_t>((part0_n / ACC_CH + nbuckets + 127) / 128, (uint64_t)ctx->sm_count * 32);
-        while (bound > 1) {
-            level_task_count_kernel<<<bb, 256, 0, st>>>(L, nbuckets);
-            scan_blocks_gated_kernel<<<nscan, SCAN_T, 0, st>>>(tcount, toff[0], toff[1], stw, scan_tmp, nbuckets);
-            scan_sums_gated_kernel<<<1, SCAN_T, 0, st>>>(scan_tmp, nscan, toff[0], toff[1], stw, nbuckets);
-            scan_add_gated_kernel<<<nscan, SCAN_T, 0, st>>>(toff[0], toff[1], stw, scan_tmp, nbuckets);
-            msm_acc_levelN_kernel<<<lv_blocks, 128, 0, st>>>(L, nbuckets);
-            level_advance_kernel<<<1, 1, 0, st>>>(L, nbuckets);
-            ctx->launches += 6;
-            bound = (bound + ACC_CH - 1) / ACC_CH;
-        }
+    ctx->launches += 2;
+    // each level >= 1 exits at once when the lists are already single
+    const LevelBufs L = {{b.toff[0], b.toff[1]}, {b.part[0], b.part[1]}, b.tcount, b.state};
+    const unsigned lv_blocks = (unsigned)std::min<uint64_t>((p.part0_n / ACC_CH + p.nbuckets + 127) / 128, (uint64_t)ctx->sm_count * 32);
+    for (uint32_t lv = 0; lv < p.acc_levels; ++lv) {
+        level_task_count_kernel<<<bb, 256, 0, st>>>(L, p.nbuckets);
+        exclusive_scan_u32<true>(ctx, b.tcount, b.toff[0], b.toff[1], (const uint32_t *)b.state, p.nbuckets, b.scan_tmp, st);
+        msm_acc_levelN_kernel<<<lv_blocks, 128, 0, st>>>(L, p.nbuckets);
+        level_advance_kernel<<<1, 1, 0, st>>>(L, p.nbuckets);
+        ctx->launches += 3;
     }
-    msm_gather_buckets_kernel<<<bb, 256, 0, st>>>(L, nbuckets, buckets);
+    msm_gather_buckets_kernel<<<bb, 256, 0, st>>>(L, p.nbuckets, b.buckets);
     ctx->launches++;
+    return ZKB_OK;
+}
 
-    // window reduction by levels
-    {
-        const G1Xyzz *in = buckets;
-        uint32_t count = half;
-        G1Xyzz *p = lvl;
-        for (uint32_t lv = 0; lv < nlevels; ++lv) {
-            const uint32_t segs = (count + (1u << log_l) - 1) >> log_l;
-            G1Xyzz *acc_out = p, *run_out = p + (size_t)segs * m.windows;
-            msm_wsum_level_kernel<<<(m.windows * segs + 127) / 128, 128, 0, st>>>(in, count, log_l, m.windows, acc_out, run_out);
-            uint32_t wt = 32;
-            while (wt < segs && wt < 256) wt <<= 1;
-            msm_window_sum_kernel<<<m.windows, wt, wt * sizeof(G1Xyzz), st>>>(acc_out, lvl_sums + (size_t)lv * m.windows, segs);
-            ctx->launches += 2;
-            in = run_out;
-            count = segs;
-            p += 2ull * segs * m.windows;
-            if (lv + 1 == nlevels) {
-                // count == 1 now: run_out[w] is the sum of all buckets of window w
-                ZKB_CUDA(cudaMemcpyAsync(all_sum, run_out, (size_t)m.windows * sizeof(G1Xyzz), cudaMemcpyDeviceToDevice, st));
-            }
-        }
-        msm_window_combine_kernel<<<(m.windows + 31) / 32, 32, 0, st>>>(lvl_sums, all_sum, nlevels, log_l, m.windows, wres);
-        ctx->launches++;
+// window reduction: per reduction window sum_j j * bucket_j by levels of running sums, then the combine
+static int32_t msm_reduce_windows(zkb_ctx *ctx, const MsmPlan &p, const MsmBufs &b, cudaStream_t st) {
+    const uint32_t W = p.wred;
+    const G1Xyzz *in = b.buckets;
+    uint32_t count = p.m.half;
+    G1Xyzz *out = b.lvl;
+    for (uint32_t lv = 0; lv < p.nlevels; ++lv) {
+        const uint32_t segs = (count + (1u << p.log_l) - 1) >> p.log_l;
+        G1Xyzz *acc_out = out, *run_out = out + (size_t)segs * W;
+        msm_wsum_level_kernel<<<(W * segs + 127) / 128, 128, 0, st>>>(in, count, p.log_l, W, acc_out, run_out);
+        uint32_t wt = 32;
+        while (wt < segs && wt < 256) wt <<= 1;
+        msm_window_sum_kernel<<<W, wt, wt * sizeof(G1Xyzz), st>>>(acc_out, b.lvl_sums + (size_t)lv * W, segs);
+        ctx->launches += 2;
+        in = run_out;
+        count = segs;
+        out += 2ull * segs * W;
     }
+    // count == 1 now: the last level's run_out[w] is the sum of all buckets of window w
+    ZKB_CUDA(cudaMemcpyAsync(b.all_sum, in, (size_t)W * sizeof(G1Xyzz), cudaMemcpyDeviceToDevice, st));
+    msm_window_combine_kernel<<<(W + 31) / 32, 32, 0, st>>>(b.lvl_sums, b.all_sum, p.nlevels, p.log_l, W, b.wres);
+    ctx->launches++;
     ZKB_CUDA(cudaGetLastError());
+    return ZKB_OK;
+}
 
-    std::vector<G1Xyzz> h(m.windows);
+// on the host: Horner over each column's window sums (W * c doublings + W additions of single points), and the counters
+static int32_t msm_finish(zkb_ctx *ctx, const MsmPlan &p, const MsmBufs &b, G1Affine *out_host, cudaStream_t st) {
+    std::vector<G1Xyzz> h(p.wred);
     MsmState h_state;
     uint32_t total_pairs = 0;
-    ZKB_CUDA(cudaMemcpyAsync(h.data(), wres, m.windows * sizeof(G1Xyzz), cudaMemcpyDeviceToHost, st));
-    ZKB_CUDA(cudaMemcpyAsync(&h_state, d_state, sizeof(MsmState), cudaMemcpyDeviceToHost, st));
-    ZKB_CUDA(cudaMemcpyAsync(&total_pairs, offsets + nbuckets, 4, cudaMemcpyDeviceToHost, st));
+    ZKB_CUDA(cudaMemcpyAsync(h.data(), b.wres, p.wred * sizeof(G1Xyzz), cudaMemcpyDeviceToHost, st));
+    ZKB_CUDA(cudaMemcpyAsync(&h_state, b.state, sizeof(MsmState), cudaMemcpyDeviceToHost, st));
+    ZKB_CUDA(cudaMemcpyAsync(&total_pairs, b.offsets + p.nbuckets, 4, cudaMemcpyDeviceToHost, st));
     ZKB_CUDA(cudaStreamSynchronize(st));   // the ONLY synchronisation of an MSM: its result is needed on the host (transcript)
-    // Horner over windows on the host (W * c doublings + W additions of single points), per column
-    for (uint32_t col = 0; col < batch; ++col) {
-        const G1Xyzz *hw = h.data() + (size_t)col * rwin1;
-        G1Xyzz acc = hw[rwin1 - 1];
-        for (int w = (int)rwin1 - 2; w >= 0; --w) {
-            for (uint32_t k = 0; k < m.c; ++k) acc = g1_dbl(acc);
+    for (uint32_t col = 0; col < p.batch; ++col) {
+        const G1Xyzz *hw = h.data() + (size_t)col * p.sets;
+        G1Xyzz acc = hw[p.sets - 1];
+        for (int w = (int)p.sets - 2; w >= 0; --w) {
+            for (uint32_t k = 0; k < p.m.c; ++k) acc = g1_dbl(acc);
             g1_add(acc, hw[w]);
         }
-        out_affine_host[col] = g1_to_affine(acc);
+        out_host[col] = g1_to_affine(acc);
     }
-    ctx->msm_last_adds = (uint64_t)total_pairs + h_state.extra_adds + 2ull * nbuckets;
+    ctx->msm_last_adds = (uint64_t)total_pairs + h_state.extra_adds + 2ull * p.nbuckets;
     ctx->msm_last_levels = h_state.levels_run;
     return ZKB_OK;
 }
 
-int32_t msm_g1_device(zkb_ctx *ctx, const Fr *scalars, const G1Affine *bases, uint64_t n, G1Affine *out_affine_host, cudaStream_t st) {
-    if (n == 0) {
-        memset(out_affine_host, 0, sizeof(G1Affine));
+// d_cols: DEVICE array of `batch` device pointers
+static int32_t msm_pass(zkb_ctx *ctx, const Fr *const *d_cols, uint32_t batch, const G1Affine *bases, uint64_t n, G1Affine *out_host,
+                        bool shifted, cudaStream_t st) {
+    MsmPlan p;
+    MsmBufs b;
+    ZKB_TRY(msm_plan(n, batch, shifted, &p));
+    ZKB_TRY(msm_scratch(ctx, p, &b));
+    ZKB_TRY(msm_sort(ctx, p, b, d_cols, st));
+    ZKB_TRY(msm_accumulate(ctx, p, b, bases, st));
+    ZKB_TRY(msm_reduce_windows(ctx, p, b, st));
+    return msm_finish(ctx, p, b, out_host, st);
+}
+
+int32_t msm_g1_columns(zkb_ctx *ctx, const Fr *const *h_cols, uint32_t count, const G1Affine *bases, uint64_t n, G1Affine *out_host,
+                       bool shifted, cudaStream_t st) {
+    if (n == 0) {   // msm_last_levels keeps the previous MSM's value
+        memset(out_host, 0, sizeof(G1Affine) * count);
         ctx->msm_last_adds = 0;
         return ZKB_OK;
     }
+    const uint32_t maxb = msm_max_batch(n);
     const Fr **d_tbl = nullptr;
     ZKB_TRY(scratch_get(ctx, SCR_MSM_TBL, 64 * sizeof(Fr *), (void **)&d_tbl));
-    ZKB_CUDA(cudaMemcpyAsync(d_tbl, &scalars, sizeof(Fr *), cudaMemcpyHostToDevice, st));
-    return msm_g1_batch_device(ctx, d_tbl, 1, bases, n, out_affine_host, st);
+    for (uint32_t done = 0; done < count; done += maxb) {
+        const uint32_t cur = std::min(count - done, maxb);
+        ZKB_CUDA(cudaMemcpyAsync(d_tbl, h_cols + done, cur * sizeof(Fr *), cudaMemcpyHostToDevice, st));
+        ZKB_TRY(msm_pass(ctx, d_tbl, cur, bases, n, out_host + done, shifted, st));
+    }
+    return ZKB_OK;
 }
 
-}  // namespace zkb
-using namespace zkb;
+int32_t msm_g1_device(zkb_ctx *ctx, const Fr *scalars, const G1Affine *bases, uint64_t n, G1Affine *out_affine_host, cudaStream_t st) {
+    return msm_g1_columns(ctx, &scalars, 1, bases, n, out_affine_host, false, st);
+}
 
-static void emit_outputs(const G1Affine &r, uint64_t out_affine[8], uint64_t *out_jacobian, uint8_t *out_compressed) {
+void g1_emit(const G1Affine &r, uint64_t out_affine[8], uint64_t *out_jacobian, uint8_t *out_compressed) {
     memcpy(out_affine, &r, 64);
     if (out_jacobian) {
         memcpy(out_jacobian, &r, 64);
@@ -622,13 +632,16 @@ static void emit_outputs(const G1Affine &r, uint64_t out_affine[8], uint64_t *ou
     if (out_compressed) g1_compress(r, out_compressed);
 }
 
+}  // namespace zkb
+using namespace zkb;
+
 extern "C" int32_t zkb_msm_g1_dev(zkb_ctx *ctx, const uint64_t *scalars_dev, const uint64_t *bases_dev, uint64_t n, uint64_t out_affine[8],
                                   uint64_t *out_jacobian, uint8_t *out_compressed, void *stream) {
     ZKB_ARG(ctx && out_affine && (n == 0 || (scalars_dev && bases_dev)));
     ZKB_CUDA(cudaSetDevice(ctx->device));
     G1Affine r;
     ZKB_TRY(msm_g1_device(ctx, (const Fr *)scalars_dev, (const G1Affine *)bases_dev, n, &r, pick_stream(ctx, stream)));
-    emit_outputs(r, out_affine, out_jacobian, out_compressed);
+    g1_emit(r, out_affine, out_jacobian, out_compressed);
     return ZKB_OK;
 }
 
@@ -650,16 +663,8 @@ extern "C" int32_t zkb_msm_g1_batch_dev(zkb_ctx *ctx, const uint64_t *const *sca
                                         uint64_t *out_affine, void *stream) {
     ZKB_ARG(ctx && scalar_cols_dev && bases_dev && out_affine && batch >= 1);
     ZKB_CUDA(cudaSetDevice(ctx->device));
-    cudaStream_t st = pick_stream(ctx, stream);
-    const uint32_t maxb = msm_max_batch(n);
-    for (uint32_t done = 0; done < batch; done += maxb) {
-        const uint32_t cur = batch - done < maxb ? batch - done : maxb;
-        const Fr **d_tbl = nullptr;
-        ZKB_TRY(scratch_get(ctx, SCR_MSM_TBL, 64 * sizeof(Fr *), (void **)&d_tbl));
-        ZKB_CUDA(cudaMemcpyAsync(d_tbl, scalar_cols_dev + done, cur * sizeof(Fr *), cudaMemcpyHostToDevice, st));
-        ZKB_TRY(msm_g1_batch_device(ctx, d_tbl, cur, (const G1Affine *)bases_dev, n, (G1Affine *)out_affine + done, st));
-    }
-    return ZKB_OK;
+    return msm_g1_columns(ctx, (const Fr *const *)scalar_cols_dev, batch, (const G1Affine *)bases_dev, n, (G1Affine *)out_affine, false,
+                          pick_stream(ctx, stream));
 }
 
 extern "C" int32_t zkb_g1_fixed_base_mul_dev(zkb_ctx *ctx, const uint64_t base_affine_host[8], const uint64_t *scalars_dev, uint64_t n,

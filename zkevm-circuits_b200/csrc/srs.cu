@@ -143,18 +143,9 @@ int32_t srs_create(zkb_ctx *ctx, uint32_t k, const G1Affine *g, bool g_on_device
 // cols: HOST array of device pointers, len scalars each (len <= n; shifted copies only serve len == n).
 int32_t srs_commit_many(zkb_srs *s, int basis, const Fr *const *cols, uint32_t count, uint64_t len, G1Affine *out_host, cudaStream_t st) {
     ZKB_ARG(s && (basis == 0 || basis == 1) && len <= s->n);
-    zkb_ctx *ctx = s->ctx;
-    const G1Affine *bases = basis == 0 ? s->g : s->g_lagrange;
     const G1Affine *shift = (len == s->n) ? (basis == 0 ? s->g_shift : s->g_lagrange_shift) : nullptr;
-    const uint32_t maxb = msm_max_batch(len);
-    for (uint32_t done = 0; done < count; done += maxb) {
-        const uint32_t cur = count - done < maxb ? count - done : maxb;
-        const Fr **d_tbl = nullptr;
-        ZKB_TRY(scratch_get(ctx, SCR_MSM_TBL, 64 * sizeof(Fr *), (void **)&d_tbl));
-        ZKB_CUDA(cudaMemcpyAsync(d_tbl, cols + done, cur * sizeof(Fr *), cudaMemcpyHostToDevice, st));
-        ZKB_TRY(msm_g1_batch_device_ex(ctx, d_tbl, cur, shift ? shift : bases, len, out_host + done, shift != nullptr, st));
-    }
-    return ZKB_OK;
+    const G1Affine *bases = shift ? shift : basis == 0 ? s->g : s->g_lagrange;
+    return msm_g1_columns(s->ctx, cols, count, bases, len, out_host, shift != nullptr, st);
 }
 
 }  // namespace zkb
@@ -191,19 +182,14 @@ extern "C" int32_t zkb_srs_read(zkb_srs *srs, int32_t basis, uint64_t *out_host)
     ZKB_CUDA(cudaStreamSynchronize(srs->ctx->stream));
     return ZKB_OK;
 }
-static void srs_emit(const G1Affine &r, uint64_t out_affine[8], uint8_t *out_compressed) {
-    memcpy(out_affine, &r, 64);
-    if (out_compressed) g1_compress(r, out_compressed);
-}
 extern "C" int32_t zkb_srs_commit_dev(zkb_srs *srs, int32_t basis, const uint64_t *scalars_dev, uint64_t n, uint64_t out_affine[8], uint8_t *out_compressed,
                                       void *stream) {
     ZKB_ARG(srs && out_affine && (n == 0 || scalars_dev));
     ZKB_CUDA(cudaSetDevice(srs->ctx->device));
     G1Affine r;
     const Fr *col = (const Fr *)scalars_dev;
-    if (n == 0) memset(&r, 0, sizeof(r));
-    else ZKB_TRY(srs_commit_many(srs, basis, &col, 1, n, &r, pick_stream(srs->ctx, stream)));
-    srs_emit(r, out_affine, out_compressed);
+    ZKB_TRY(srs_commit_many(srs, basis, &col, 1, n, &r, pick_stream(srs->ctx, stream)));
+    g1_emit(r, out_affine, nullptr, out_compressed);
     return ZKB_OK;
 }
 extern "C" int32_t zkb_srs_commit_host(zkb_srs *srs, int32_t basis, const uint64_t *scalars_host, uint64_t n, uint64_t out_affine[8], uint8_t *out_compressed) {
