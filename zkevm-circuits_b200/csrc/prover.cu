@@ -961,6 +961,102 @@ static int32_t quotient_gates(const Csf &cs, const std::vector<Fr> &challenges, 
     return ZKB_OK;
 }
 
+// Lookup input sets combined in coefficient form.  compress_exprs makes an input set of W >= 2 expressions e_c into
+// sum_c theta^(W-1-c) e_c.  When every e_c is S * a_c(w^r X) -- one advice-free cofactor S (the same hash-consed node; or no
+// cofactor at all), one rotation r -- that sum is S * A(w^r X) with A = sum_c theta^(W-1-c) a_c.  A is formed once from the
+// advice polynomials and the quotient reads it as one more slot: one coset NTT per part instead of W, and per row one column
+// load and (with S) one product instead of W loads, W products and W - 1 theta steps.  The coset NTT is linear and field
+// arithmetic exact, so the values, h and the proof do not change.  A set combines only if none of its columns is read in the quotient other than through combined sets (gates,
+// the permutation, tables, sets compressed term by term): such a column keeps its coset NTTs, and A would add one.
+struct InputCombos {
+    struct Set { int32_t combo = -1; uint32_t cofactor = NO_NODE; int32_t rot = 0; };   // combo -1: compressed term by term
+    std::vector<std::vector<Set>> sets;            // [lookup][input set]
+    std::vector<std::vector<uint32_t>> columns;    // per combination, its advice columns in order: the slot sm.slots + index
+};
+static InputCombos lookup_input_combos(const Csf &cs, ExprBuilder &qeb, const SlotMap &sm, const std::vector<Fr> &challenges,
+                                       std::vector<int64_t> &memo) {
+    // nodes that read an advice or instance cell (operands come before the node that reads them)
+    std::vector<char> reads_cells(cs.nodes.size(), 0);
+    for (size_t i = 0; i < cs.nodes.size(); ++i) {
+        const auto &nd = cs.nodes[i];
+        reads_cells[i] = nd[0] == N_ADVICE || nd[0] == N_INSTANCE || (nd[0] >= N_NEG && reads_cells[nd[1]]) ||
+                         ((nd[0] == N_ADD || nd[0] == N_MUL) && reads_cells[nd[2]]);
+    }
+    std::vector<char> elsewhere(cs.na, 0), seen(cs.nodes.size(), 0);   // advice columns read other than through combined sets
+    auto read_by = [&](uint32_t root) {
+        std::vector<uint32_t> stack{root};
+        while (!stack.empty()) {
+            const uint32_t v = stack.back();
+            stack.pop_back();
+            if (seen[v]) continue;
+            seen[v] = 1;
+            const auto &nd = cs.nodes[v];
+            if (nd[0] == N_ADVICE) elsewhere[nd[1]] = 1;
+            if (nd[0] >= N_NEG) stack.push_back(nd[1]);
+            if (nd[0] == N_ADD || nd[0] == N_MUL) stack.push_back(nd[2]);
+        }
+    };
+    for (uint32_t g : cs.gates) read_by(g);
+    for (auto &pc : cs.perm)
+        if (pc[0] == N_ADVICE) elsewhere[pc[1]] = 1;
+    InputCombos out;
+    std::vector<std::vector<std::vector<uint32_t>>> cols(cs.lookups.size());   // a candidate set's columns
+    out.sets.resize(cs.lookups.size());
+    for (size_t l = 0; l < cs.lookups.size(); ++l) {
+        const CsfLookup &lk = cs.lookups[l];
+        for (uint32_t v : lk.table) read_by(v);
+        out.sets[l].resize(lk.inputs.size());
+        cols[l].resize(lk.inputs.size());
+        for (size_t i = 0; i < lk.inputs.size(); ++i) {
+            const std::vector<uint32_t> &inp = lk.inputs[i];
+            InputCombos::Set &set = out.sets[l][i];
+            bool ok = inp.size() >= 2;
+            for (size_t c = 0; c < inp.size() && ok; ++c) {
+                // e_c = Advice(col, rot), or Advice(col, rot) * S / S * Advice(col, rot) with S advice- and instance-free
+                const auto &nd = cs.nodes[inp[c]];
+                uint32_t adv = inp[c], cof = NO_NODE;
+                if (nd[0] == N_MUL) {
+                    const int side = cs.nodes[nd[1]][0] == N_ADVICE && !reads_cells[nd[2]] ? 0 : 1;
+                    adv = nd[1 + side];
+                    cof = nd[2 - side];
+                    if (reads_cells[cof]) ok = false;
+                }
+                if (!ok || cs.nodes[adv][0] != N_ADVICE) { ok = false; break; }
+                const uint32_t s = cof == NO_NODE ? NO_NODE : translate(cs, cof, qeb, sm, challenges, memo);
+                const int32_t rot = (int32_t)cs.nodes[adv][2];
+                if (c == 0) { set.cofactor = s; set.rot = rot; }
+                else ok = s == set.cofactor && rot == set.rot;
+                cols[l][i].push_back(cs.nodes[adv][1]);
+            }
+            if (ok) set.combo = 0;
+            else for (uint32_t v : inp) read_by(v);
+        }
+    }
+    // a set dropped for a column read elsewhere makes its other columns read elsewhere too
+    for (bool changed = true; changed;) {
+        changed = false;
+        for (size_t l = 0; l < cs.lookups.size(); ++l)
+            for (size_t i = 0; i < cols[l].size(); ++i) {
+                InputCombos::Set &set = out.sets[l][i];
+                if (set.combo < 0 || std::none_of(cols[l][i].begin(), cols[l][i].end(), [&](uint32_t c) { return elsewhere[c]; })) continue;
+                set.combo = -1;
+                for (uint32_t c : cols[l][i]) elsewhere[c] = 1;
+                changed = true;
+            }
+    }
+    // one combination per distinct column tuple, in order of first use
+    std::map<std::vector<uint32_t>, int32_t> index;
+    for (size_t l = 0; l < cs.lookups.size(); ++l)
+        for (size_t i = 0; i < cols[l].size(); ++i) {
+            InputCombos::Set &set = out.sets[l][i];
+            if (set.combo < 0) continue;
+            auto it = index.emplace(cols[l][i], (int32_t)out.columns.size()).first;
+            if (it->second == (int32_t)out.columns.size()) out.columns.push_back(cols[l][i]);
+            set.combo = it->second;
+        }
+    return out;
+}
+
 // evaluation.rs evaluate_h: the quotient numerator (gates, permutation, lookups, in upstream's y-Horner order) as one program per
 // degree group (QuotientGroups), then per coset part j the coset NTTs of the polynomials its groups read that the pk's coset cache
 // does not hold, and one interpreter launch per group on the part, x y^(T-1-i_last) / ((zeta w^j)^n - 1)
@@ -981,7 +1077,6 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
     put_columns(qpolys, sm.z0, ps.z_polys);
     put_columns(qpolys, sm.phi0, ps.phi_polys);
     put_columns(qpolys, sm.m0, ps.m_polys);
-    ZKB_ARG(qpolys.size() < 65536);
 
     const uint32_t E = pk->E;
     uint32_t G = 1;   // groups m = 1, 2, .., E
@@ -1008,10 +1103,20 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
             if (!qg.scope({qeb.mul(qeb.sub(left, right), lactive())})) { set_error("permutation: %s", qg.error.c_str()); return ZKB_ERR_ARG; }
         }
     }
+    const InputCombos combos = lookup_input_combos(cs, qeb, sm, s->challenges, memo);
     for (size_t l = 0; l < cs.lookups.size(); ++l) {
         const CsfLookup &lk = cs.lookups[l];
         std::vector<uint32_t> fsb;
-        for (auto &inp : lk.inputs) fsb.push_back(qeb.add(compress_exprs(cs, inp, qeb, sm, s->challenges, memo, ps.theta), qeb.constant(ps.beta)));
+        for (size_t i = 0; i < lk.inputs.size(); ++i) {
+            const InputCombos::Set &set = combos.sets[l][i];
+            uint32_t f;
+            if (set.combo < 0) f = compress_exprs(cs, lk.inputs[i], qeb, sm, s->challenges, memo, ps.theta);
+            else {
+                f = qeb.col(sm.slots + (uint32_t)set.combo, set.rot);
+                if (set.cofactor != NO_NODE) f = qeb.mul(set.cofactor, f);
+            }
+            fsb.push_back(qeb.add(f, qeb.constant(ps.beta)));
+        }
         const uint32_t tb = qeb.add(compress_exprs(cs, lk.table, qeb, sm, s->challenges, memo, ps.theta), qeb.constant(ps.beta));
         uint32_t prod = fsb[0];
         for (size_t j = 1; j < fsb.size(); ++j) prod = qeb.mul(prod, fsb[j]);
@@ -1037,6 +1142,25 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
             return ZKB_ERR_ARG;
         }
     }
+    // the combined input columns A = sum_c theta^(W-1-c) a_c in coefficient form, slots sm.slots + index.  Every rank holds every
+    // advice polynomial (coefficient_forms all-gathers them), so each forms all of them.  `coefs` lives until the stream is synchronised.
+    std::vector<std::vector<Fr>> coefs(combos.columns.size());
+    Fr *combo_polys = nullptr;
+    if (!combos.columns.empty()) ZKB_TRY(pool.fr(combos.columns.size() * n, &combo_polys));
+    for (size_t c = 0; c < combos.columns.size(); ++c) {
+        const std::vector<uint32_t> &cols = combos.columns[c];
+        std::vector<Fr *> polys(cols.size());
+        coefs[c].resize(cols.size());
+        Fr p = one;
+        for (size_t t = cols.size(); t-- > 0;) {
+            polys[t] = ps.adv_polys[cols[t]];
+            coefs[c][t] = p;
+            p = fp_mul(p, ps.theta);
+        }
+        ZKB_TRY(lincomb(pk, pool, polys, coefs[c], combo_polys + c * n, false, st));
+        qpolys.push_back(combo_polys + c * n);
+    }
+    ZKB_ARG(qpolys.size() < 65536);
     // group g runs on the coset parts j = 0 mod E/m, m = 2^g: every group on part 0, only the top one (m = E) on the odd parts
     auto on_part = [&](uint32_t g, uint32_t j) { return j % (E >> g) == 0; };
     std::vector<uint32_t> groups;   // the non-empty ones
@@ -1058,7 +1182,7 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
         ZKB_TRY(upload_program(pool, qpbs[g], qeb, qdp[g], st));
     }
     // slots served from the pk's coset cache
-    auto cached = [&](size_t i) { return !pk->coset_cache.empty() && pk->coset_cache[0][i]; };
+    auto cached = [&](size_t i) { return !pk->coset_cache.empty() && i < pk->coset_cache[0].size() && pk->coset_cache[0][i]; };
     // the largest group reading each slot: a polynomial outside the cache is transformed on that group's parts (a smaller group's
     // parts are a subset of them), and not at all when no constraint reads it
     std::vector<int> reader(qpolys.size(), -1);
@@ -1084,8 +1208,14 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
     trace.mark("quotient program build+upload");
 
     // evaluate h part by part: group g's value at zeta w_{mn}^(j' + m i) is h_g[j' + m i], part j = (E/m) j'; the top group's h_g is h_ext
+    // one n-element array per polynomial that is transformed; the others are read from the coset cache or by no group
+    std::vector<Fr *> qcols(qpolys.size(), nullptr);
+    size_t transformed = 0;
+    for (size_t i = 0; i < qpolys.size(); ++i) transformed += !cached(i) && reader[i] >= 0;
     Fr *slab, *pows;
-    ZKB_TRY(pool.fr(qpolys.size() * n, &slab));
+    ZKB_TRY(pool.fr(transformed * n, &slab));
+    for (size_t i = 0, t = 0; i < qpolys.size(); ++i)
+        if (!cached(i) && reader[i] >= 0) qcols[i] = slab + t++ * n;
     ZKB_TRY(pool.fr(n, &pows));
     ZKB_TRY(pool.fr(pk->N, &ps.h_ext));
     ps.h_group.assign(G, nullptr);
@@ -1093,8 +1223,6 @@ static int32_t evaluate_h(zkb_session *s, ProofState &ps, StageTrace &trace) {
         if (g + 1 == G) ps.h_group[g] = ps.h_ext;
         else ZKB_TRY(pool.fr(n << g, &ps.h_group[g]));
     }
-    std::vector<Fr *> qcols(qpolys.size());
-    for (size_t i = 0; i < qpolys.size(); ++i) qcols[i] = slab + i * n;
     // multi-GPU: coset parts are dealt in contiguous blocks.  A rank writes one n-element row of rows_slab per (part, group on it),
     // parts in order from row rank * blk_rows, so one all-gather of blk_rows rows per rank completes the slab; each group's rows are
     // then interleaved into its order h_g[j' + m i]
