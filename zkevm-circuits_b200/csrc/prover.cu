@@ -648,8 +648,8 @@ struct ProofState {
     Fr *h_ext = nullptr;                     // h on the extended domain; after the inverse transform, qdeg pieces of n coefficients
     std::vector<Fr *> h_group;               // quotient group g's values on zeta D_{mn}, m = 2^g (the top one is h_ext; null: empty)
     std::vector<Fr *> h_pieces;
-    std::map<int64_t, Fr> point_of;          // rotation -> x * omega^rot
-    std::map<std::pair<int, int64_t>, Fr> eval_of;
+    std::map<int64_t, Fr> point_of;          // rotation mod n -> x * omega^rot
+    std::map<std::pair<int, int64_t>, Fr> eval_of;   // (polynomial, rotation mod n) -> evaluation
     std::vector<OpenQuery> queries;          // multiopen queries in prover.rs order
 };
 
@@ -1340,6 +1340,9 @@ static int32_t evaluate_at_x(zkb_session *s, ProofState &ps) {
     for (auto &v : m_id) v = next_id++;
     const int h_id = next_id++, rand_id = next_id++;
     const int64_t rot_last = -(int64_t)(cs.bf + 1);
+    // rotations r and r + n open a polynomial at the same point (omega^n = 1): SHPLONK's sets are sets of points
+    // (construct_intermediate_sets compares point values), so the opening side keys every rotation by r mod n
+    const auto at = [n](int64_t rot) { return ((rot % (int64_t)n) + (int64_t)n) % (int64_t)n; };
     // (1) the evaluations written to the transcript, in order; `queries` is built afterwards in the multiopen order
     struct EvalReq { int poly_id; const Fr *poly; int64_t rot; };
     std::vector<EvalReq> reqs;
@@ -1365,7 +1368,7 @@ static int32_t evaluate_at_x(zkb_session *s, ProofState &ps) {
     std::vector<Fr> evals(reqs.size());
     for (auto &kv : by_rot) {
         const Fr pt = fp_mul(ps.x, fr_pow_i64(pk->omega, pk->omega_inv, kv.first));
-        ps.point_of[kv.first] = pt;
+        ps.point_of[at(kv.first)] = pt;
         std::vector<Fr *> ptrs;
         for (size_t i : kv.second) ptrs.push_back(const_cast<Fr *>(reqs[i].poly));
         Fr **d_p = nullptr;
@@ -1388,10 +1391,10 @@ static int32_t evaluate_at_x(zkb_session *s, ProofState &ps) {
         for (size_t t = 0; t < kv.second.size(); ++t) evals[kv.second[t]] = res[t];
     }
     for (size_t i = 0; i < n_written; ++i) s->tr.write_scalar(evals[i]);
-    for (size_t i = 0; i < reqs.size(); ++i) ps.eval_of[{reqs[i].poly_id, reqs[i].rot}] = evals[i];
+    for (size_t i = 0; i < reqs.size(); ++i) ps.eval_of[{reqs[i].poly_id, at(reqs[i].rot)}] = evals[i];
 
     // (2) multiopen queries in prover.rs order
-    auto push_q = [&](int id, const Fr *poly, int64_t rot) { ps.queries.push_back({id, poly, rot}); };
+    auto push_q = [&](int id, const Fr *poly, int64_t rot) { ps.queries.push_back({id, poly, at(rot)}); };
     for (auto &q : cs.advq) push_q(adv_id[q[0]], ps.adv_polys[q[0]], q[1]);
     for (uint32_t i = 0; i < pk->nsets; ++i) { push_q(z_id[i], ps.z_polys[i], 0); push_q(z_id[i], ps.z_polys[i], 1); }
     for (int i = (int)pk->nsets - 2; i >= 0; --i) push_q(z_id[i], ps.z_polys[i], rot_last);
