@@ -281,9 +281,18 @@ ZKB_API int32_t zkb_msm_g1_sharded_dev(zkb_ctx *ctx, const uint64_t *scalars_sha
  * 128-byte unique id, the host layer broadcasts it, every rank calls zkb_comm_init.  With a communicator the proving session
  * stays replicated (identical transcript and proof bytes on every rank) while independent units -- columns, lookup arguments,
  * permutation sets, the quotient's coset parts -- are cut into P contiguous blocks (rank r computes block r) and each result is
- * completed by one in-place all-gather.                                                                                      */
+ * completed by one in-place all-gather.  At most 16 ranks.                                                                    */
 ZKB_API int32_t zkb_comm_unique_id(uint8_t out[128]);
 ZKB_API int32_t zkb_comm_init(zkb_ctx *ctx, const uint8_t unique_id[128], int32_t rank, int32_t nranks);
+/* zkb_comm_init_local   joins `nranks` contexts of ONE process on ONE device into one group (context i becomes rank i), so the
+ *                       multi-rank paths run on a single GPU: each rank is then driven from its own host thread.  The collectives
+ *                       stay stream-ordered (events, device-to-device copies; no host synchronisation is added).  Every collective
+ *                       carries its kind and size: ranks that disagree all fail with ZKB_ERR_STATE before anything is copied.  A
+ *                       meeting of the ranks that waits longer than timeout_ms poisons the group: every later collective fails at
+ *                       once with ZKB_ERR_STATE.  ZKB_ERR_ARG: 1 <= nranks <= 16 violated, contexts on different devices, a context
+ *                       given twice or one that already has a communicator.  zkb_comm_destroy / zkb_destroy of any member ends the
+ *                       group for the others (their next collective fails).                                                        */
+ZKB_API int32_t zkb_comm_init_local(zkb_ctx *const *ctxs, int32_t nranks, uint32_t timeout_ms);
 ZKB_API int32_t zkb_comm_destroy(zkb_ctx *ctx);
 
 /* ---- create_proof: device-resident proving session --------------------------------------------------------------

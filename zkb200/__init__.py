@@ -6,4 +6,4 @@ import os as _os
 
 __path__.append(_os.path.join(_os.path.dirname(_os.path.dirname(_os.path.abspath(__file__))), "zkevm-circuits_b200"))
 
-from .lib import ZkbError, load_library, Context, default_context  # noqa: E402,F401
+from .lib import ZkbError, load_library, Context, default_context, init_comm_local  # noqa: E402,F401

@@ -69,10 +69,12 @@ struct zkb_ctx {
     cudaStream_t copy_stream = nullptr;  // H2D of witness columns overlaps the MSMs of the previous batch
     int sm_count = 132;
     size_t mem_bytes = 0;   // device memory (cudaDeviceProp::totalGlobalMem): the default budgets of the optional caches scale with it
-    // multi-GPU: NCCL communicator of this rank (comm.cu); nranks == 1 -> everything local
+    // multi-GPU: communicator of this rank (comm.cu), NCCL or in-process (several contexts of one process on one device, each
+    // driven from its own thread); nranks == 1 -> everything local
     void *nccl_comm = nullptr;
+    void *local_comm = nullptr;
     int rank = 0, nranks = 1;
-    // peer-memory exchange window of this rank (sharded.cu): cudaMalloc'ed, exported with cudaIpc, mapped by every other rank
+    // peer-memory exchange window of this rank (comm.cu): cudaMalloc'ed, mapped by every other rank (cudaIpc, or shared in-process)
     void *win_local = nullptr;
     size_t win_bytes = 0;
     void *win_peers[16] = {nullptr};   // win_peers[rank] == win_local
@@ -192,7 +194,7 @@ int32_t comm_allgather(zkb_ctx *ctx, const void *send, void *recv, size_t bytes_
 int32_t comm_alltoall(zkb_ctx *ctx, const void *send, void *recv, size_t bytes_per_block, cudaStream_t st);
 // stream-ordered barrier across the ranks (a 8-byte all-reduce): work queued before it on every rank is complete when it completes
 int32_t comm_barrier(zkb_ctx *ctx, cudaStream_t st);
-// peer-memory window of at least `bytes` on every rank, mapped into every rank (cudaIpc); COLLECTIVE, same `bytes` everywhere
+// peer-memory window of at least `bytes` on every rank, mapped into every rank; COLLECTIVE, same `bytes` everywhere
 int32_t comm_window(zkb_ctx *ctx, size_t bytes, cudaStream_t st);
 
 struct DevPool {  // owns device allocations of a pk / session; blocks are recycled through the context's block cache

@@ -1,4 +1,5 @@
 // expr.cu -- device interpreter for constraint-expression programs (see expr.cuh).
+#include <atomic>
 #include <type_traits>
 #include "common.cuh"
 #include "expr.cuh"
@@ -167,12 +168,14 @@ __global__ void __launch_bounds__(THREADS) expr_flag_kernel(FlagLaunch L) {
 template <class Launch, int NREGS, int THREADS, void (*KERNEL)(Launch)>
 static int32_t launch_smem(const Launch &L, uint32_t n, cudaStream_t st) {
     constexpr size_t bytes = (size_t)NREGS * THREADS * 32;
-    static bool attr_set[64] = {};
+    // the opt-in is per device; contexts of one process may launch from several threads at the same time.  Setting it is
+    // idempotent, so threads that both find the flag clear both set it; the flag is published only after the attribute is set
+    static std::atomic<bool> attr_set[64];
     int dev = 0;
     cudaGetDevice(&dev);
-    if (bytes > 48 * 1024 && dev < 64 && !attr_set[dev]) {
+    if (bytes > 48 * 1024 && dev < 64 && !attr_set[dev].load(std::memory_order_acquire)) {
         ZKB_CUDA(cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-        attr_set[dev] = true;
+        attr_set[dev].store(true, std::memory_order_release);
     }
     KERNEL<<<(n + THREADS - 1) / THREADS, THREADS, bytes, st>>>(L);
     return ZKB_OK;

@@ -551,16 +551,15 @@ static int32_t get_plan(zkb_ctx *ctx, uint32_t log_n, const Fr &omega, NttPlan *
 // ---- tensor maps ------------------------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *,
                                   const cuuint32_t *, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// resolved once: a function-local static is initialised exactly once, also when several threads start their first transform together
 static EncodeTiledFn encode_tiled_fn() {
-    static EncodeTiledFn fn = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
+    static const EncodeTiledFn fn = []() -> EncodeTiledFn {
         void *p = nullptr;
         cudaDriverEntryPointQueryResult qres;
         if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess && qres == cudaDriverEntryPointSuccess)
-            fn = (EncodeTiledFn)p;
-    }
+            return (EncodeTiledFn)p;
+        return nullptr;
+    }();
     return fn;
 }
 // 2-D view of one column for a pass with row stride S = 2^log_inner elements: dim0 = S * 4 u64 (one row of S elements), dim1 = n / S rows;

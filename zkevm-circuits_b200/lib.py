@@ -74,6 +74,7 @@ SIGNATURES = {
     "zkb_msm_g1_sharded_dev": (ctypes.c_int32, [_vp, _vp, _vp, ctypes.c_uint64, _vp, _vp, _vp]),
     "zkb_comm_unique_id": (ctypes.c_int32, [_vp]),
     "zkb_comm_init": (ctypes.c_int32, [_vp, _vp, ctypes.c_int32, ctypes.c_int32]),
+    "zkb_comm_init_local": (ctypes.c_int32, [ctypes.POINTER(_vp), ctypes.c_int32, ctypes.c_uint32]),
     "zkb_comm_destroy": (ctypes.c_int32, [_vp]),
     "zkb_pk_create": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, _vp, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
     "zkb_pk_create_with_srs": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, _vp, _vp, _vp, ctypes.POINTER(_vp)]),
@@ -182,6 +183,15 @@ class Context:
 
     def sync(self):
         check(self.lib.zkb_sync(self.handle))
+
+
+def init_comm_local(ctxs, timeout_ms=60000):
+    """Join the contexts `ctxs` (one process, one device) into one in-process group: ctxs[i] becomes rank i of len(ctxs).  Drive each
+    rank from its own thread afterwards; ctypes releases the GIL during every call into the library, so Python threads are enough.
+    A collective that waits more than timeout_ms for the other ranks fails with ZkbError, and so does every later one of the group."""
+    ctxs = list(ctxs)
+    arr = (_vp * max(1, len(ctxs)))(*[c.handle for c in ctxs])
+    check(load_library().zkb_comm_init_local(arr, len(ctxs), int(timeout_ms)))
 
 
 _default = {}
