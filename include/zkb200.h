@@ -343,7 +343,10 @@ ZKB_API int32_t zkb_pk_destroy(zkb_pk *pk);
 /* VerifyingKey bytes in SerdeFormat::Processed layout (u32 BE k || u32 BE num_fixed || fixed || permutation commitments,
  * compressed points; the layout of the reference fixture's vk).  out may be NULL to query the length.                     */
 ZKB_API int32_t zkb_pk_vk_bytes(zkb_pk *pk, uint8_t *out, uint64_t cap, uint64_t *len);
-/* Host-only structural validation of a CSF blob (no CUDA device needed); zkb_pk_create runs it first.                       */
+/* Host-only structural validation of a CSF blob (no CUDA device needed); zkb_pk_create, zkb_pk_create_with_srs and
+ * zkb_keygen_pk run it first.  Deviation from halo2: SHPLONK opens one advice or fixed column at the points x w^r of its
+ * distinct rotations mod n, and this prover takes at most 256 such points per column (upstream has no limit).  A CSF that
+ * opens a column at more fails here with ZKB_ERR_ARG, naming the column and its point count; rotations r and r -+ n count once. */
 ZKB_API int32_t zkb_csf_validate(const uint32_t *csf, uint64_t csf_words);
 /* The gates of a CSF evaluated over caller columns by the prover's own expression compiler and interpreter (the quotient's hot
  * kernel, exposed for row-by-row tests).  columns_dev: HOST array of device pointers in slot order fixed | advice | instance,

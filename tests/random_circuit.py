@@ -26,6 +26,8 @@ MAX_ROT = 9                 # |rotation| of gates and lookups, except the occasi
 MAX_ROTS_PER_COLUMN = 5     # distinct rotations of one advice column: blinding factors <= 7, usable >= n - 8
 MAX_DEPTH = 4               # DAG depth of a random expression: its program stays far below the interpreter's 64 registers
 MAX_DEGREE = 17             # cs.degree() <= 17: extended factor E <= 16
+MAX_ROT_BITS = 32767        # the interpreter keeps a rotation in 16 bits (csrc/csf.cuh)
+MAX_POINTS_PER_COLUMN = 256  # SHPLONK opens one column at most at this many points (zkb_csf_validate)
 
 
 @dataclasses.dataclass
@@ -45,6 +47,10 @@ class Shape:
     n_cycles: int           # copy cycles
     far_rotation: bool      # gates read rotations +-(n - 1); one column is read at both r and r -+ n (r = +-1)
     transcript: str
+    # ((kind, points, rotations), ...): one gate reads a free "fixed" or "advice" column at `rotations` rotation numbers that
+    # make `points` distinct points mod n (rotations - points of them are r -+ n of another); the columns' point sets are
+    # disjoint.  An advice column's blinding factors become its query count + 2.  Never drawn: only overrides set it.
+    wide_columns: tuple = ()
 
     @staticmethod
     def draw(rnd):
@@ -150,6 +156,9 @@ class RandomCircuit:
         self.shape = sh = dataclasses.replace(shape, **overrides)
         self.k, self.n = sh.k, 1 << sh.k
         n = self.n
+        if sh.far_rotation and n - 1 > MAX_ROT_BITS:
+            raise ValueError(f"far_rotation reads rotations +-(n - 1) = +-{n - 1} at k = {sh.k}: the interpreter keeps a rotation "
+                             f"in 16 bits (|rotation| <= {MAX_ROT_BITS}), so far_rotation needs k <= 15")
         self.transcript = sh.transcript
         self.fixed_role, self.adv_role, self.adv_phase, self._rots = [], [], [], []
         self.challenge_phase = [p for p in range(sh.phases - 1) for _ in range(rnd.randint(1, 2))]
@@ -165,7 +174,7 @@ class RandomCircuit:
         cs = H.ConstraintSystem(self.k, len(self.fixed_role), len(self.adv_role), sh.n_instance, list(self.adv_phase), list(self.challenge_phase))
         cs.gates, cs.lookups = gates, lookups
         pool = [(ADVICE, c) for c in self.free] * 2 + [(FIXED, c) for c in self.free_fixed] + [(INSTANCE, i) for i in range(sh.n_instance)] \
-            + [(ADVICE, c) for c in range(len(self.adv_role)) if c not in self.free]
+            + [(ADVICE, c) for c in range(len(self.adv_role)) if c not in self.free and self.adv_role[c] != "wide"]
         perm = []
         for col in rnd.sample(pool, len(pool)):
             if len(perm) < sh.n_perm and col not in perm:
@@ -177,7 +186,7 @@ class RandomCircuit:
         assert 3 <= self.degree <= MAX_DEGREE, self.degree
         self.bf = bf = cs.blinding_factors()
         self.usable = usable = n - (bf + 1)
-        assert bf <= MAX_ROTS_PER_COLUMN + 2
+        assert bf <= max([MAX_ROTS_PER_COLUMN] + [rots for kind, _, rots in sh.wide_columns if kind == "advice"]) + 2
         self._values()
         chunk = self.degree - 2
         nsets = (len(perm) + chunk - 1) // chunk
@@ -404,12 +413,41 @@ class RandomCircuit:
                 body = x - _rewrite(x, rnd)
             self.identities.append(len(gates))
             gates.append(H.fixed(sel) * body if sel is not None else body)
+        used = set()
+        for kind, points, rotations in sh.wide_columns:
+            gates.append(self._wide_gate(kind, points, rotations, used, len(gates)))
         order = list(range(len(gates)))
         rnd.shuffle(order)
         where = {g: i for i, g in enumerate(order)}
         self.derived = [(d, where[g], sel, p) for d, g, sel, p in self.derived]
         self.identities = [where[g] for g in self.identities]
         return [gates[g] for g in order]
+
+    def _wide_gate(self, kind, points, rotations, used, gate):
+        """q * (d - sum_i c_i col(r_i)) over a fresh column read at `rotations` rotation numbers that make `points` points mod n,
+        none of them in `used`; d is a derived column"""
+        rnd, n = self.rnd, self.n
+        assert kind in ("fixed", "advice") and 1 <= points <= rotations < 2 * points, (kind, points, rotations)
+        rots = rnd.sample([r for r in range(-(n // 2) + 1, n // 2 + 1) if r % n not in used], points)
+        used.update(r % n for r in rots)
+        rots += [r - n if r > 0 else r + n for r in rnd.sample([r for r in rots if r], rotations - points)]
+        assert all(abs(r) <= MAX_ROT_BITS for r in rots)
+        phase = rnd.randrange(self.shape.phases)
+        if kind == "advice":
+            col = self._advice("wide", phase)
+            self._rots[col] = set(rots)
+            read = H.advice
+        else:
+            col = self._fixed("wide")
+            read = H.fixed
+
+        def total(xs):
+            return xs[0] if len(xs) == 1 else total(xs[: len(xs) // 2]) + total(xs[len(xs) // 2:])
+        p = total([H.scaled(read(col, r), rnd.randrange(1, R)) for r in rots])
+        d = self._advice("derived", phase)
+        sel = rnd.choice(self.selectors)
+        self.derived.append((d, gate, sel, p))
+        return H.fixed(sel) * (H.advice(d) - p)
 
     # ------------------------------------------------------------------------------------------------ values
     def _values(self):
@@ -421,11 +459,11 @@ class RandomCircuit:
             elif role == "qt":
                 fixed[c] = [int(rnd.random() < 0.7) for i in range(n)]
                 fixed[c][rnd.randrange(usable)] = 0           # the zero tuple is a table row
-            elif role == "free":
+            elif role in ("free", "wide"):
                 fixed[c] = [self._value() for _ in range(n)]
         adv = [None] * len(self.adv_role)
         for c, role in enumerate(self.adv_role):
-            if role in ("free", "table"):
+            if role in ("free", "table", "wide"):
                 adv[c] = [self._value() for _ in range(n)]
         self.instances = []
         for i in range(sh.n_instance):
@@ -581,7 +619,7 @@ class RandomCircuit:
                 f"fixed={cs.num_fixed} advice={cs.num_advice} instance={cs.num_instance} gates={len(cs.gates)} "
                 f"(derived {len(self.derived)}, unselected {sum(s is None for _, _, s, _ in self.derived)}, identity {len(self.identities)}) "
                 f"lookups=[{lks}] perm={len(cs.perm_columns)} cols/{-(-len(cs.perm_columns) // chunk)} sets copies={len(self.copies)} "
-                f"bf={self.bf} transcript={self.transcript}")
+                f"bf={self.bf} transcript={self.transcript}" + (f" wide={list(self.shape.wide_columns)}" if self.shape.wide_columns else ""))
 
 
 def _copy(e):

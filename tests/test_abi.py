@@ -113,6 +113,31 @@ def test_csf_rotation_limit():
                     Z.validate_csf(cs.to_csf())
 
 
+
+@pytest.mark.parametrize("kind", ["fixed", "advice"])
+def test_csf_opening_point_limit(kind):
+    """SHPLONK opens one column at most at 256 points x w^r (distinct rotations mod n): 256 are accepted, 257 are refused with the
+    column and its count, 257 rotations of which two are equal mod n (r and r - n) make 256 points and are accepted."""
+    import zkb200
+    from zkb200 import plonk as Z
+    E = Z.Expression
+    k = 10
+    n = 1 << k
+    for rots, ok in ((list(range(-128, 128)), True), (list(range(-128, 129)), False), (list(range(-128, 128)) + [100 - n], True)):
+        cs = Z.ConstraintSystem(k, 2, 2, 0, [0, 0], [], len(rots) + 2 if kind == "advice" else 5, 3)
+        read = E.Fixed if kind == "fixed" else E.Advice
+        body = read(1, rots[0])
+        for r in rots[1:]:
+            body = body + read(1, r)
+        cs.gates = [E.Fixed(0) * (E.Advice(0) + body)]
+        queries = [(0, 0), (1, 0)] + [(1, r) for r in rots if r != 0]
+        cs.advice_queries, cs.fixed_queries = ([(0, 0)] + queries[1:], [(0, 0)]) if kind == "advice" else ([(0, 0)], queries)
+        if ok:
+            Z.validate_csf(cs.to_csf())
+        else:
+            with pytest.raises(zkb200.ZkbError, match=f"{kind} column 1 is opened at 257 points"):
+                Z.validate_csf(cs.to_csf())
+
 def test_params_file_roundtrip(tmp_path, oracle):
     """ParamsKZG file layout of the reference loader (prover/src/utils.rs:56-75): 4 B k | g | g_lagrange | g2 | s_g2, RawBytes."""
     import numpy as np

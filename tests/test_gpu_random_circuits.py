@@ -36,10 +36,11 @@ def assert_same_proof(tc, proof, proof_ref, what="proof"):
                 f"'{item_at(layout, i)}' (32-byte word {first_diff(proof, proof_ref)}); {tc.describe()}")
 
 
-def prove_and_compare(tc, monkeypatch, again=False):
+def prove_and_compare(tc, monkeypatch, again=False, oracle=None):
+    """oracle: (ref, pkr, proof, verified) of oracle_prove(tc, tc.transcript) when the caller has it already"""
     from zkb200 import plonk as Z
     from zkb200.params import ParamsKZG
-    ref, pkr, proof_ref, ok = oracle_prove(tc, tc.transcript)
+    ref, pkr, proof_ref, ok = oracle if oracle is not None else oracle_prove(tc, tc.transcript)
     assert ok, f"the oracle rejects its own proof: {tc.describe()}"
     F = ref.F
     fixed = [F.arr(c) for c in tc.fixed_ints]

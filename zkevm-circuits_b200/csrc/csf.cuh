@@ -3,6 +3,7 @@
 // Host code, shared by the prover (prover.cu), the lookup compression (lookup.cu) and the witness check (check.cu).
 #pragma once
 #include <string.h>
+#include <algorithm>
 #include "common.cuh"
 #include "expr.cuh"
 
@@ -118,6 +119,29 @@ inline int32_t load_csf(const uint32_t *csf, uint64_t csf_words, Csf &c) {
     for (uint32_t ph : c.adv_phase) if (ph >= c.nphases) { set_error("CSF: advice phase out of range"); return ZKB_ERR_ARG; }
     for (uint32_t ph : c.ch_phase) if (ph >= c.nphases) { set_error("CSF: challenge phase out of range"); return ZKB_ERR_ARG; }
     return ZKB_OK;
+}
+
+// SHPLONK opens a column at the points x w^r of its distinct rotations mod n, and the prover takes at most MAX_POINTS_PER_COLUMN
+// of them (shplonk() in prover.cu); instance columns are not opened.  The point sets are static in the CSF, so zkb_csf_validate
+// and every pk constructor refuse a constraint system past the limit before any proof work.
+constexpr size_t MAX_POINTS_PER_COLUMN = 256;
+inline int32_t check_openings(const Csf &c) {
+    const int64_t n = 1ll << c.k;
+    auto chk = [&](const std::vector<std::array<int32_t, 2>> &q, uint32_t ncols, const char *what) {
+        std::vector<std::vector<int64_t>> pts(ncols);
+        for (auto &e : q) pts[e[0]].push_back(((e[1] % n) + n) % n);
+        for (uint32_t col = 0; col < ncols; ++col) {
+            std::sort(pts[col].begin(), pts[col].end());
+            const size_t m = std::unique(pts[col].begin(), pts[col].end()) - pts[col].begin();
+            if (m > MAX_POINTS_PER_COLUMN) {
+                set_error("CSF: %s column %u is opened at %zu points (distinct rotations mod n), more than the %zu SHPLONK takes per column",
+                          what, col, m, MAX_POINTS_PER_COLUMN);
+                return false;
+            }
+        }
+        return true;
+    };
+    return chk(c.advq, c.na, "advice") && chk(c.fixq, c.nf, "fixed") ? ZKB_OK : ZKB_ERR_ARG;
 }
 
 // the caller's `nch` challenge values (4 limbs each, Montgomery form)

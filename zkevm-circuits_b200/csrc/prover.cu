@@ -47,7 +47,7 @@ __global__ void scale_const_kernel(Fr *__restrict__ a, Fr c, uint64_t n) {
 }
 // out[i] -= low[i] for i < k (subtract a low-degree polynomial given on the device)
 __global__ void sub_low_kernel(Fr *__restrict__ out, const Fr *__restrict__ low, uint32_t k) {
-    uint32_t i = threadIdx.x;   // one block of 256 threads: a rotation set has at most 256 points
+    uint32_t i = threadIdx.x;   // one block of MAX_POINTS_PER_COLUMN threads: a rotation set has at most that many points
     if (i < k) fp_store(out + i, fp_sub(fp_load(out + i), fp_load(low + i)));
 }
 
@@ -340,6 +340,7 @@ extern "C" int32_t zkb_pk_create(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf
     ZKB_CUDA(cudaSetDevice(ctx->device));
     Csf cs;
     ZKB_TRY(load_csf(csf, csf_words, cs));
+    ZKB_TRY(check_openings(cs));
     zkb_srs *srs = nullptr;
     ZKB_TRY(srs_create(ctx, cs.k, (const G1Affine *)g, false, (const G1Affine *)g_lagrange, false, &srs));
     const int32_t r = pk_build(ctx, std::move(cs), fixed_values, sigma_values, nullptr, srs, true, out);
@@ -351,6 +352,7 @@ extern "C" int32_t zkb_pk_create_with_srs(zkb_ctx *ctx, const uint32_t *csf, uin
     ZKB_ARG(ctx && csf && srs && out);
     Csf cs;
     ZKB_TRY(load_csf(csf, csf_words, cs));
+    ZKB_TRY(check_openings(cs));
     return pk_build(ctx, std::move(cs), fixed_values, sigma_values, nullptr, srs, false, out);
 }
 
@@ -370,6 +372,7 @@ extern "C" int32_t zkb_keygen_pk(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf
     ZKB_CUDA(cudaSetDevice(ctx->device));
     Csf cs;
     ZKB_TRY(load_csf(csf, csf_words, cs));
+    ZKB_TRY(check_openings(cs));
     const uint64_t n = 1ull << cs.k;
     const size_t P = cs.perm.size();
     ZKB_ARG(P * n < (1ull << 32));
@@ -454,7 +457,8 @@ extern "C" int32_t zkb_pk_vk_bytes(zkb_pk *pk, uint8_t *out, uint64_t cap, uint6
 // host-only structural check of a CSF blob (no device needed)
 extern "C" int32_t zkb_csf_validate(const uint32_t *csf, uint64_t csf_words) {
     Csf c;
-    return load_csf(csf, csf_words, c);
+    ZKB_TRY(load_csf(csf, csf_words, c));
+    return check_openings(c);
 }
 
 extern "C" int32_t zkb_pk_destroy(zkb_pk *pk) {
@@ -1469,7 +1473,7 @@ static int32_t shplonk(zkb_session *s, ProofState &ps) {
     ZKB_TRY(pool.fr(n, &hx));
     ZKB_TRY(pool.fr(n, &work));
     ZKB_TRY(pool.fr(n, &work2));
-    ZKB_TRY(pool.fr(256, &d_small));
+    ZKB_TRY(pool.fr(MAX_POINTS_PER_COLUMN, &d_small));
     ZKB_CUDA(cudaMemsetAsync(hx, 0, n * sizeof(Fr), st));
     std::vector<std::vector<std::vector<Fr>>> r_coeffs(rsets.size());   // [set][commitment] -> interpolant R_ij
     Fr vpow = one;
@@ -1477,7 +1481,7 @@ static int32_t shplonk(zkb_session *s, ProofState &ps) {
         const RSet &rs = rsets[si];
         std::vector<Fr> pts;
         for (int64_t r : rs.rots) pts.push_back(ps.point_of[r]);
-        ZKB_ARG(pts.size() <= 256);   // Keccak's hot cell column is opened at 56 rotations (keccak_packed_multi.rs:59-68)
+        ZKB_ARG(pts.size() <= MAX_POINTS_PER_COLUMN);   // refused earlier by check_openings; Keccak's hot cell column has 56 points
         // N_i(X) = sum_j y^j (P_ij(X) - R_ij(X))
         std::vector<Fr *> ptrs;
         std::vector<Fr> cf;
@@ -1494,7 +1498,7 @@ static int32_t shplonk(zkb_session *s, ProofState &ps) {
         }
         ZKB_TRY(lincomb(pk, pool, ptrs, cf, work, false, st));
         ZKB_CUDA(cudaMemcpyAsync(d_small, rsum.data(), rsum.size() * sizeof(Fr), cudaMemcpyHostToDevice, st));
-        sub_low_kernel<<<1, 256, 0, st>>>(work, d_small, (uint32_t)rsum.size());
+        sub_low_kernel<<<1, MAX_POINTS_PER_COLUMN, 0, st>>>(work, d_small, (uint32_t)rsum.size());
         ctx->launches++;
         ZKB_CUDA(cudaStreamSynchronize(st));
         // divide by the vanishing polynomial of the set, one root at a time
