@@ -189,6 +189,58 @@ ZKB_API int32_t zkb_g1_encode(zkb_ctx *ctx, int32_t format, const uint64_t *in_a
 ZKB_API int32_t zkb_g2_decode_host(int32_t format, const uint8_t *in, uint64_t out[16], int32_t *status);
 ZKB_API int32_t zkb_g2_encode_host(int32_t format, const uint64_t in[16], uint8_t *out);
 
+/* ---- proving-key files: ProvingKey::write / ProvingKey::read (halo2_proofs plonk.rs, PSE line) ----------------------------------------
+ * snark-verifier-sdk's gen_pk(params, circuit, Some(path)) caches keys on disk with these two functions.  A pk file is, in order:
+ *   vk      u32 BE k || u32 BE num_fixed || fixed commitments || permutation commitments; points 32 B compressed (Processed) or the
+ *           raw 64 B G1Affine (RawBytes, RawBytesUnchecked), as zkb_g1_encode encodes them.  No selector bytes: the CSF carries no
+ *           selectors.  A caller whose halo2 appends packed selectors to the vk writes / consumes those bytes itself, between the vk
+ *           section and the body.
+ *   body    sections 0 l0, 1 l_last, 2 l_active_row (one polynomial each, extended form, N = 2^ext_k values), 3 fixed_values (n each),
+ *           4 fixed_polys (coefficients, n each), 5 fixed_cosets (extended, N each), 6 permutation sigma values (n each), 7 their
+ *           coefficient forms (n each), 8 their extended forms (N each).  Sections 3 - 8 are slices: u32 BE count, then polynomials.
+ *           A polynomial is u32 BE length, then its elements.  Extended index m is the value at zeta * omega_ext^m (coeff_to_extended),
+ *           i.e. coset part m mod E, row m / E of the prover's coset layout.  l_active_row = 1 - l_last - l_blind.
+ *   Fr      32 B: Processed = canonical little-endian (< r); RawBytes = the Montgomery limbs, stored integer < r; RawBytesUnchecked =
+ *           the Montgomery limbs, not checked.
+ * I/O goes through caller callbacks, the read_exact / write_all of Rust's io::Read / io::Write: the library never seeks and never
+ * holds a whole file.  read() returns 0 when all len bytes were read, ZKB_IO_EOF when the input ended first (a truncated file:
+ * ZKB_ERR_ARG naming the section) and any other non-zero value on an I/O error; write() returns 0 or non-zero.  Any other non-zero
+ * callback return aborts the call with ZKB_ERR_STATE.
+ * zkb_pk_vk_write  the vk section in `format`; Processed gives exactly the bytes of zkb_pk_vk_bytes.  COLLECTIVE like zkb_pk_vk_bytes.
+ * zkb_pk_write     sections 0 - 8.  Values and coefficient forms come from the key; extended forms from the coset cache when it holds
+ *                  them, otherwise they are computed column by column into one N x 32 B scratch from the context's block cache.  The
+ *                  encode kernel gathers the E coset parts in extended order and encodes chunk by chunk (ZKB_SERDE_CHUNK_POINTS
+ *                  elements) through pinned double buffers.  The same key gives the same bytes on every run.  Rank-local.
+ * zkb_pk_read      sections 0 - 8 of a key for `csf` (the caller has consumed the vk section and checked k and num_fixed).  Every
+ *                  length prefix is checked against the CSF's n, N, num_fixed and permutation column count before anything is
+ *                  allocated for it.  Fixed and sigma values are decoded on the GPU and the key is built by the same stages as
+ *                  zkb_pk_create_with_srs (same coset-cache decision, same proof bytes).  The derived sections (0 - 2, 4, 5, 7, 8) are
+ *                  decoded too: with check = 0 they are range-checked (per format) and discarded; with check = 1 every element is also
+ *                  compared, in the decode kernel, with the form the key being built derives.  Deviation from upstream, which trusts the
+ *                  file's polys and cosets: here they are never loaded, only checked or skipped.  Reading stops at the end of the
+ *                  first polynomial that holds a bad element; *rep then names it: section, column (0 for sections 0 - 2), the index of
+ *                  its first bad element, the number of bad elements in it and the reason of the first (ZKB_SERDE_NON_CANONICAL or
+ *                  ZKB_PK_MISMATCH).  Bad elements, wrong length prefixes and truncated input return ZKB_ERR_ARG and no key; *rep is
+ *                  filled on every return: after a wrong length prefix or truncated input it names where reading stopped (column
+ *                  UINT32_MAX for a slice's count) with reason 0 and count 0; after success section and column are UINT32_MAX
+ *                  (first_index UINT64_MAX, count 0).  The context stays usable.  COLLECTIVE on a context with a communicator: every rank reads its own copy of
+ *                  the file, and when any rank fails every rank returns ZKB_ERR_ARG.                                                */
+#define ZKB_IO_EOF 1
+#define ZKB_PK_MISMATCH 4   /* check = 1: a derived element differs from the form the key derives */
+typedef struct zkb_io_vtable {
+    void *user;
+    int32_t (*read)(void *user, uint8_t *buf, uint64_t len);
+    int32_t (*write)(void *user, const uint8_t *buf, uint64_t len);
+} zkb_io_vtable;
+typedef struct zkb_pk_read_report {
+    uint32_t section, column, reason, reserved;
+    uint64_t first_index, count;
+} zkb_pk_read_report;
+ZKB_API int32_t zkb_pk_vk_write(struct zkb_pk *pk, int32_t format, const zkb_io_vtable *io);
+ZKB_API int32_t zkb_pk_write(struct zkb_pk *pk, int32_t format, const zkb_io_vtable *io);
+ZKB_API int32_t zkb_pk_read(zkb_ctx *ctx, const uint32_t *csf, uint64_t csf_words, int32_t format, const zkb_io_vtable *io, zkb_srs *srs,
+                            int32_t check, zkb_pk_read_report *rep, struct zkb_pk **out);
+
 /* ---- element-wise field kernels (device buffers); field: 0 = Fr, 1 = Fq ------------------------------------
  * op: 0 add, 1 sub, 2 mul (binary);  unary op: 0 invert (0 -> 0), 1 canonical->Montgomery, 2 Montgomery->canonical,
  * 3 square, 4 negate.  These back Polynomial +,-,* and the unit tests of the device arithmetic.                  */

@@ -1,4 +1,4 @@
-//! Raw bindings of include/zkb200.h (ABI version 1.5).  Field elements and points cross as `*const u64` / `*mut u64`:
+//! Raw bindings of include/zkb200.h (ABI version 1.7).  Field elements and points cross as `*const u64` / `*mut u64`:
 //! halo2curves' `Fr`, `Fq` are `#[repr(transparent)]` over `[u64; 4]` (Montgomery form) and `G1Affine` is `{ x: Fq, y: Fq }`, so
 //! `slice.as_ptr() as *const u64` needs no conversion (layout checked against the reference fixture in tests/test_oracle_golden.py).
 #![allow(non_camel_case_types)]
@@ -17,6 +17,22 @@ pub struct zkb_check_record { pub kind: u32, pub index: u32, pub sub: u32, pub r
 /// 3 not on the curve)
 #[repr(C)] #[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
 pub struct zkb_decode_report { pub first_bad: u64, pub count: u64, pub reason: u32, pub reserved: u32 }
+
+/// `R: io::Read` / `W: io::Write` of ProvingKey::read / write as read_exact / write_all callbacks (see plonk/pk_serde_gpu.rs); read
+/// returns ZKB_IO_EOF when the input ends first
+#[repr(C)]
+pub struct zkb_io_vtable {
+    pub user: *mut c_void,
+    pub read: unsafe extern "C" fn(user: *mut c_void, buf: *mut u8, len: u64) -> i32,
+    pub write: unsafe extern "C" fn(user: *mut c_void, buf: *const u8, len: u64) -> i32,
+}
+pub const ZKB_IO_EOF: i32 = 1;
+pub const ZKB_PK_MISMATCH: u32 = 4;
+
+/// outcome of zkb_pk_read: where reading stopped (section 0 - 8, column; u32::MAX when every element is good), reason of the first bad
+/// element (2 not canonical, 4 ZKB_PK_MISMATCH), its index in the polynomial and the number of bad elements in it
+#[repr(C)] #[derive(Clone, Copy, Debug, Default, PartialEq, Eq)]
+pub struct zkb_pk_read_report { pub section: u32, pub column: u32, pub reason: u32, pub reserved: u32, pub first_index: u64, pub count: u64 }
 
 /// create_proof's generic `T: TranscriptWrite` as four C callbacks (see gpu/transcript.rs)
 #[repr(C)]
@@ -51,6 +67,11 @@ extern "C" {
     pub fn zkb_g1_encode(ctx: *mut zkb_ctx, format: i32, in_affine: *const u64, n: u64, out: *mut u8, stream: *mut c_void) -> i32;
     pub fn zkb_g2_decode_host(format: i32, input: *const u8, out: *mut u64, status: *mut i32) -> i32;
     pub fn zkb_g2_encode_host(format: i32, input: *const u64, out: *mut u8) -> i32;
+    // proving-key files
+    pub fn zkb_pk_vk_write(pk: *mut zkb_pk, format: i32, io: *const zkb_io_vtable) -> i32;
+    pub fn zkb_pk_write(pk: *mut zkb_pk, format: i32, io: *const zkb_io_vtable) -> i32;
+    pub fn zkb_pk_read(ctx: *mut zkb_ctx, csf: *const u32, csf_words: u64, format: i32, io: *const zkb_io_vtable, srs: *mut zkb_srs,
+                       check: i32, rep: *mut zkb_pk_read_report, out: *mut *mut zkb_pk) -> i32;
     // ParamsKZG::setup / unsafe_setup_with_s / new (s: Montgomery Fr < r; outputs 2^k G1Affine each, device buffers)
     pub fn zkb_srs_setup_dev(ctx: *mut zkb_ctx, k: u32, s: *const u64, g_out_dev: *mut u64, g_lagrange_out_dev: *mut u64,
                              stream: *mut c_void) -> i32;

@@ -21,6 +21,7 @@
 #include "csf.cuh"
 #include "expr.cuh"
 #include "lookup.cuh"
+#include "pk.cuh"
 #include "transcript.cuh"
 #include <algorithm>
 #include <memory>
@@ -73,30 +74,6 @@ static Fr fr_pow_i64(const Fr &base, const Fr &base_inv, int64_t e) { return e >
 
 }  // namespace zkb
 using namespace zkb;
-
-struct zkb_pk {
-    zkb_ctx *ctx = nullptr;
-    Csf cs;
-    SlotMap sm;
-    uint32_t k = 0, ext_k = 0, E = 0, qdeg = 0, chunk = 0, nsets = 0;
-    uint64_t n = 0, N = 0;
-    Fr omega, omega_inv, ext_omega, ext_omega_inv, n_inv, N_inv, zeta;
-    std::vector<Fr> t_inv;
-    DevPool pool;
-    std::vector<Fr *> fixed_values, fixed_polys, sigma_values, sigma_polys;
-    Fr *l0_poly = nullptr, *llast_poly = nullptr, *lblind_poly = nullptr, *xid_poly = nullptr, *omega_pows = nullptr;
-    zkb_srs *srs = nullptr;       // shared ParamsKZG handle (owned when the pk was made by the legacy zkb_pk_create)
-    bool owns_srs = false;
-    // coset evaluations of the proof-independent polynomials (fixed, sigma, X, l_0, l_last, l_blind) for every coset part, like
-    // upstream's pk.fixed_cosets / permutation cosets / l0 / l_last / l_active_row: [part][slot] -> n elements, null for the other
-    // slots; empty when the cache is off
-    std::vector<std::vector<Fr *>> coset_cache;
-    ~zkb_pk() {
-        if (owns_srs && srs) zkb_srs_destroy(srs);
-    }
-    // generator zeta * ext_omega^j of coset part j
-    Fr coset_gen(uint32_t j) const { return fp_mul(zeta, fp_pow_u64(ext_omega, j)); }
-};
 
 struct zkb_session {
     zkb_pk *pk = nullptr;
@@ -225,7 +202,7 @@ static int32_t lincomb(zkb_pk *pk, DevPool &pool, const std::vector<Fr *> &polys
 
 // ================================================================================================ C ABI: proving key
 // the quotient table's proof-independent slots in coefficient form, null elsewhere
-static std::vector<Fr *> pk_quotient_polys(const zkb_pk *pk) {
+std::vector<Fr *> zkb::pk_quotient_polys(const zkb_pk *pk) {
     const SlotMap &sm = pk->sm;
     std::vector<Fr *> t(sm.slots, nullptr);
     put_columns(t, sm.fixed0, pk->fixed_polys);
@@ -234,19 +211,16 @@ static std::vector<Fr *> pk_quotient_polys(const zkb_pk *pk) {
     return t;
 }
 
-// Builds the device-resident proving key of a loaded CSF.  sigma columns come either from the host (sigma_values) or are already on
-// the device (sigma_dev, keygen path).  The SRS handle is shared, not copied.
-static int32_t pk_build(zkb_ctx *ctx, Csf &&csf, const uint64_t *const *fixed_values, const uint64_t *const *sigma_values,
-                        const std::vector<Fr *> *sigma_dev, zkb_srs *srs, bool owns_srs, zkb_pk **out) {
+// The first stage of every pk constructor: domain constants, l_0 / l_last / l_blind / X in coefficient form, omega^i.  The SRS handle
+// is shared, not copied.
+int32_t zkb::pk_begin(zkb_ctx *ctx, Csf &&csf, zkb_srs *srs, zkb_pk **out) {
     ZKB_CUDA(cudaSetDevice(ctx->device));
     std::unique_ptr<zkb_pk> pk(new zkb_pk());
     pk->ctx = ctx;
     pk->pool.ctx = ctx;
     pk->srs = srs;
-    pk->owns_srs = owns_srs;
     pk->cs = std::move(csf);
     const Csf &cs = pk->cs;
-    ZKB_ARG((cs.nf == 0 || fixed_values) && (cs.perm.empty() || sigma_values || sigma_dev));
     if (srs->ctx != ctx || srs->k != cs.k) { set_error("the SRS handle is for k = %u on another context or size (circuit k = %u): downsize it first", srs->k, cs.k); return ZKB_ERR_ARG; }
     cudaStream_t st = ctx->stream;
     pk->k = cs.k;
@@ -272,22 +246,6 @@ static int32_t pk_build(zkb_ctx *ctx, Csf &&csf, const uint64_t *const *fixed_va
     pk->zeta = host_zeta();
     pk->t_inv.resize(pk->E);
     for (uint32_t j = 0; j < pk->E; ++j) pk->t_inv[j] = fp_inv(fp_sub(fp_pow_u64(pk->coset_gen(j), n), Fr::one()));
-    // fixed / sigma columns: values and coefficient form (sources on the host, or on the device for keygen's sigma)
-    auto ingest = [&](const void *const *src, size_t cnt, std::vector<Fr *> &vals, std::vector<Fr *> &polys) -> int32_t {
-        vals.resize(cnt);
-        polys.resize(cnt);
-        for (size_t i = 0; i < cnt; ++i) {
-            ZKB_TRY(pk->pool.fr(n, &vals[i]));
-            ZKB_TRY(pk->pool.fr(n, &polys[i]));
-            ZKB_CUDA(cudaMemcpyAsync(vals[i], src[i], n * sizeof(Fr), cudaMemcpyDefault, st));
-            ZKB_TRY(lagrange_to_coeff(pk.get(), vals[i], polys[i], st));
-        }
-        return ZKB_OK;
-    };
-    ZKB_TRY(ingest((const void *const *)fixed_values, cs.nf, pk->fixed_values, pk->fixed_polys));
-    if (sigma_dev) ZKB_ARG(sigma_dev->size() == cs.perm.size());
-    const void *const *sigma_src = sigma_dev ? (const void *const *)sigma_dev->data() : (const void *const *)sigma_values;
-    ZKB_TRY(ingest(sigma_src, cs.perm.size(), pk->sigma_values, pk->sigma_polys));
     // l_0, l_last, l_blind (Lagrange indicator vectors -> coefficient form), X (identity polynomial), omega^i
     ZKB_TRY(pk->pool.fr(n, &pk->l0_poly));
     ZKB_TRY(pk->pool.fr(n, &pk->llast_poly));
@@ -308,10 +266,33 @@ static int32_t pk_build(zkb_ctx *ctx, Csf &&csf, const uint64_t *const *fixed_va
     ZKB_TRY(lagrange_to_coeff(pk.get(), pk->llast_poly, pk->llast_poly, st));
     ZKB_TRY(lagrange_to_coeff(pk.get(), pk->lblind_poly, pk->lblind_poly, st));
     ZKB_TRY(fr_powers_device(ctx, pk->omega, n, pk->omega_pows, st));
+    *out = pk.release();
+    return ZKB_OK;
+}
+
+// fixed / sigma columns: values and coefficient form (sources on the host, or on the device)
+int32_t zkb::pk_ingest(zkb_pk *pk, const void *const *src, size_t cnt, std::vector<Fr *> &vals, std::vector<Fr *> &polys) {
+    const uint64_t n = pk->n;
+    cudaStream_t st = pk->ctx->stream;
+    vals.resize(cnt);
+    polys.resize(cnt);
+    for (size_t i = 0; i < cnt; ++i) {
+        ZKB_TRY(pk->pool.fr(n, &vals[i]));
+        ZKB_TRY(pk->pool.fr(n, &polys[i]));
+        ZKB_CUDA(cudaMemcpyAsync(vals[i], src[i], n * sizeof(Fr), cudaMemcpyDefault, st));
+        ZKB_TRY(lagrange_to_coeff(pk, vals[i], polys[i], st));
+    }
+    return ZKB_OK;
+}
+
+int32_t zkb::pk_finish(zkb_pk *pk) {
+    zkb_ctx *ctx = pk->ctx;
+    cudaStream_t st = ctx->stream;
+    const uint64_t n = pk->n;
     {
         // cache the coset evaluations of the static polynomials unless that would take more than ZKB_COSET_CACHE_GB (default: a
         // quarter of the device memory, 20 GB on an 80 GB H100 -- the rest holds the proving session's columns and coset parts)
-        const std::vector<Fr *> stat = pk_quotient_polys(pk.get());
+        const std::vector<Fr *> stat = pk_quotient_polys(pk);
         const size_t nstat = stat.size() - std::count(stat.begin(), stat.end(), nullptr);
         const char *env = getenv("ZKB_COSET_CACHE_GB");
         const double budget = env ? atof(env) * 1e9 : 0.25 * (double)ctx->mem_bytes;
@@ -324,12 +305,30 @@ static int32_t pk_build(zkb_ctx *ctx, Csf &&csf, const uint64_t *const *fixed_va
                 for (size_t i = 0; i < stat.size(); ++i) {
                     if (!stat[i]) continue;
                     ZKB_TRY(pk->pool.fr(n, &pk->coset_cache[j][i]));
-                    ZKB_TRY(ntt_fr_device(ctx, stat[i], pk->coset_cache[j][i], cs.k, pk->omega, nullptr, 0, pows, st));
+                    ZKB_TRY(ntt_fr_device(ctx, stat[i], pk->coset_cache[j][i], pk->k, pk->omega, nullptr, 0, pows, st));
                 }
             }
         }
     }
     ZKB_CUDA(cudaStreamSynchronize(st));
+    return ZKB_OK;
+}
+
+// Builds the device-resident proving key of a loaded CSF.  sigma columns come either from the host (sigma_values) or are already on
+// the device (sigma_dev, keygen path).
+static int32_t pk_build(zkb_ctx *ctx, Csf &&csf, const uint64_t *const *fixed_values, const uint64_t *const *sigma_values,
+                        const std::vector<Fr *> *sigma_dev, zkb_srs *srs, bool owns_srs, zkb_pk **out) {
+    ZKB_ARG((csf.nf == 0 || fixed_values) && (csf.perm.empty() || sigma_values || sigma_dev));
+    if (sigma_dev) ZKB_ARG(sigma_dev->size() == csf.perm.size());
+    zkb_pk *raw = nullptr;
+    ZKB_TRY(pk_begin(ctx, std::move(csf), srs, &raw));
+    std::unique_ptr<zkb_pk> pk(raw);   // owns_srs stays false until the key is complete: on failure the caller still owns the handle
+    const Csf &cs = pk->cs;
+    ZKB_TRY(pk_ingest(pk.get(), (const void *const *)fixed_values, cs.nf, pk->fixed_values, pk->fixed_polys));
+    const void *const *sigma_src = sigma_dev ? (const void *const *)sigma_dev->data() : (const void *const *)sigma_values;
+    ZKB_TRY(pk_ingest(pk.get(), sigma_src, cs.perm.size(), pk->sigma_values, pk->sigma_polys));
+    ZKB_TRY(pk_finish(pk.get()));
+    pk->owns_srs = owns_srs;
     *out = pk.release();
     return ZKB_OK;
 }
@@ -430,6 +429,16 @@ extern "C" int32_t zkb_pk_sigma_read(zkb_pk *pk, uint32_t column, uint64_t *out_
     return ZKB_OK;
 }
 
+int32_t zkb::pk_vk_commitments(zkb_pk *pk, std::vector<G1Affine> &out) {
+    ZKB_CUDA(cudaSetDevice(pk->ctx->device));
+    std::vector<Fr *> cols;
+    for (auto c : pk->fixed_values) cols.push_back(c);
+    for (auto c : pk->sigma_values) cols.push_back(c);
+    out.clear();
+    if (!cols.empty()) ZKB_TRY(commit_many(pk, cols, BASIS_LAGRANGE, out, pk->ctx->stream));
+    return ZKB_OK;
+}
+
 // VerifyingKey::write(SerdeFormat::Processed) (halo2_proofs plonk.rs): u32 BE k || u32 BE num_fixed || fixed commitments ||
 // permutation commitments, points compressed -- the layout of the reference fixture's `vk` (aggregator/data/batch-task.json:
 // 0x19, 4, 4 + 3 points = 232 B).  Commitments = commit_lagrange of the fixed / sigma columns (keygen.rs), batched MSMs.
@@ -440,13 +449,8 @@ extern "C" int32_t zkb_pk_vk_bytes(zkb_pk *pk, uint8_t *out, uint64_t cap, uint6
     *len = need;
     if (!out) return ZKB_OK;
     ZKB_ARG(cap >= need);
-    ZKB_CUDA(cudaSetDevice(pk->ctx->device));
-    cudaStream_t st = pk->ctx->stream;
-    std::vector<Fr *> cols;
-    for (auto c : pk->fixed_values) cols.push_back(c);
-    for (auto c : pk->sigma_values) cols.push_back(c);
     std::vector<G1Affine> cms;
-    if (!cols.empty()) ZKB_TRY(commit_many(pk, cols, BASIS_LAGRANGE, cms, st));
+    ZKB_TRY(pk_vk_commitments(pk, cms));
     auto be32 = [](uint8_t *p, uint32_t v) { p[0] = (uint8_t)(v >> 24); p[1] = (uint8_t)(v >> 16); p[2] = (uint8_t)(v >> 8); p[3] = (uint8_t)v; };
     be32(out, cs.k);
     be32(out + 4, cs.nf);

@@ -9,12 +9,11 @@
 // reason) lowered with atomicMin, so the report is the same on every run whatever the schedule.  Host buffers are streamed through
 // pinned double buffers in chunks of ZKB_SERDE_CHUNK_POINTS: the copy in of chunk i + 1 overlaps the kernel and the copy out of chunk i.
 #include "common.cuh"
+#include "serde.cuh"
 #include <string.h>
 #include <algorithm>
 
 namespace zkb {
-
-constexpr uint32_t SERDE_THREADS = 256;
 
 // (q + 1) / 4 = (q >> 2) + 1 (q = 3 mod 4; the + 1 cannot carry out of limb 0)
 constexpr uint32_t sqrt_exp_word(int i) {
@@ -127,34 +126,6 @@ __global__ void __launch_bounds__(SERDE_THREADS) g1_encode_processed_kernel(cons
     out[2 * i] = make_uint4(x.l[0], x.l[1], x.l[2], x.l[3]);
     out[2 * i + 1] = make_uint4(x.l[4], x.l[5], x.l[6], x.l[7]);
 }
-
-static bool is_device_ptr(const void *p) {
-    cudaPointerAttributes a;
-    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
-        cudaGetLastError();
-        return false;
-    }
-    return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
-}
-
-// The chunked pipeline of a host-side buffer: two slots, each with its own stream, pinned staging and device staging.
-struct SerdePipe {
-    zkb_ctx *ctx;
-    DevPool pool;
-    cudaStream_t s[2] = {nullptr, nullptr};
-    cudaEvent_t done[2] = {nullptr, nullptr};
-    uint8_t *h_in[2] = {nullptr, nullptr}, *h_out[2] = {nullptr, nullptr};
-    uint8_t *d_in[2] = {nullptr, nullptr}, *d_out[2] = {nullptr, nullptr};
-    explicit SerdePipe(zkb_ctx *c) : ctx(c) { pool.ctx = c; }
-    ~SerdePipe() {
-        for (int j = 0; j < 2; ++j) {
-            if (s[j]) { cudaStreamSynchronize(s[j]); cudaStreamDestroy(s[j]); }
-            if (done[j]) cudaEventDestroy(done[j]);
-            if (h_in[j]) cudaFreeHost(h_in[j]);
-            if (h_out[j]) cudaFreeHost(h_out[j]);
-        }
-    }
-};
 
 // Runs launch(src_dev, dst_dev, count, first_index, stream) over n points of in_sz bytes in / out_sz bytes out.  Device buffers on
 // both sides: one launch on st.  Otherwise host sides are staged chunk by chunk; work already queued on st is complete before the first

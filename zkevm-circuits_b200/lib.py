@@ -58,6 +58,9 @@ SIGNATURES = {
     "zkb_g1_encode": (ctypes.c_int32, [_vp, ctypes.c_int32, _vp, ctypes.c_uint64, _vp, _vp]),
     "zkb_g2_decode_host": (ctypes.c_int32, [ctypes.c_int32, _vp, _vp, ctypes.POINTER(ctypes.c_int32)]),
     "zkb_g2_encode_host": (ctypes.c_int32, [ctypes.c_int32, _vp, _vp]),
+    "zkb_pk_vk_write": (ctypes.c_int32, [_vp, ctypes.c_int32, _vp]),
+    "zkb_pk_write": (ctypes.c_int32, [_vp, ctypes.c_int32, _vp]),
+    "zkb_pk_read": (ctypes.c_int32, [_vp, _vp, ctypes.c_uint64, ctypes.c_int32, _vp, _vp, ctypes.c_int32, _vp, ctypes.POINTER(_vp)]),
     "zkb_field_binop_dev": (ctypes.c_int32, [_vp, ctypes.c_int32, ctypes.c_int32, _vp, _vp, _vp, ctypes.c_uint64, _vp]),
     "zkb_field_unop_dev": (ctypes.c_int32, [_vp, ctypes.c_int32, ctypes.c_int32, _vp, _vp, ctypes.c_uint64, _vp]),
     "zkb_fr_batch_invert_dev": (ctypes.c_int32, [_vp, _vp, _vp, ctypes.c_uint64, _vp]),

@@ -6,7 +6,9 @@ Here a constraint system is described by plain Python objects (the Rust shim wou
 `ConstraintSystem` the same way, see INTEGRATION.md) and flattened into the CSF blob documented in include/zkb200.h.
 Nothing in this module computes field arithmetic on the CPU; it only marshals buffers.
 """
+import contextlib
 import ctypes
+import os
 import struct
 from collections import namedtuple
 
@@ -367,6 +369,63 @@ class ProvingKey:
         check(self.ctx.lib.zkb_pk_vk_bytes(self.handle, ctypes.cast(out, _vp), n.value, ctypes.byref(n)))
         return bytes(out)
 
+    def vk_write(self, fmt=None):
+        """VerifyingKey::write(fmt) without selectors (zkb_pk_vk_write) -> bytes; Processed equals vk_bytes()."""
+        from .params import SerdeFormat
+        fmt = SerdeFormat.RawBytesUnchecked if fmt is None else SerdeFormat(fmt)
+        out = []
+        io = _CallbackIo(writer=lambda b: out.append(bytes(b)))
+        check(self.ctx.lib.zkb_pk_vk_write(self.handle, int(fmt), ctypes.cast(ctypes.pointer(io.vt), _vp)))
+        return b"".join(out)
+
+    def write(self, path_or_file, fmt=None):
+        """ProvingKey::write(writer, fmt): the vk section, then l0, l_last, l_active_row, the fixed values / polys / cosets and the
+        permutation values / polys / cosets (layout: include/zkb200.h).  path_or_file: a path, or a binary file object with write().
+        The default format is snark-verifier-sdk gen_pk's RawBytesUnchecked."""
+        from .params import SerdeFormat
+        fmt = SerdeFormat.RawBytesUnchecked if fmt is None else SerdeFormat(fmt)
+        with _binary_file(path_or_file, "wb") as f:
+            f.write(self.vk_write(fmt))
+            io = _CallbackIo(writer=f.write)
+            io.run(self.ctx.lib.zkb_pk_write(self.handle, int(fmt), ctypes.cast(ctypes.pointer(io.vt), _vp)))
+
+    @classmethod
+    def read(cls, path_or_file, cs, srs, fmt=None, check=False):
+        """ProvingKey::read(reader, fmt) for constraint system `cs` against the SRS handle `srs` (params.Srs of degree cs.k).
+
+        The vk header (k, num_fixed) is checked against cs; the vk commitments are recomputed from the values, and with check=True they
+        must equal the file's.  The file's polys and cosets are never loaded: with check=False they are only range-checked, with
+        check=True every element must equal the form the key derives.  Raises ZkbError; when the body is at fault the error carries
+        .report, a PkReadReport naming the section, column, first bad index, count and reason."""
+        from .params import SerdeFormat
+        fmt = SerdeFormat.RawBytesUnchecked if fmt is None else SerdeFormat(fmt)
+        ctx = srs.ctx
+        npts = cs.num_fixed + len(cs.perm_columns)
+        with _binary_file(path_or_file, "rb") as f:
+            head = _read_exact(f, 8 + npts * fmt.g1_len, "the vk section")
+            k, nf = struct.unpack(">II", head[:8])
+            if (k, nf) != (cs.k, cs.num_fixed):
+                raise ZkbError(f"pk file: the vk is for k = {k} with {nf} fixed columns, the constraint system has k = {cs.k} and {cs.num_fixed}")
+            blob = cs.to_csf()
+            rep = _PkReadReport()
+            io = _CallbackIo(reader=f)
+            h = _vp()
+            rc = ctx.lib.zkb_pk_read(ctx.handle, _vp(blob.ctypes.data), blob.size, int(fmt), ctypes.cast(ctypes.pointer(io.vt), _vp), srs.handle,
+                                     1 if check else 0, ctypes.byref(rep), ctypes.byref(h))
+            report = None if rep.count == 0 and rep.section == 0xFFFFFFFF else PkReadReport(
+                int(rep.section), int(rep.column), int(rep.reason), int(rep.first_index), int(rep.count))
+            try:
+                io.run(rc)
+            except ZkbError as e:
+                e.report = report
+                raise
+        pk = cls.__new__(cls)
+        pk.ctx, pk.cs, pk.srs, pk.handle = ctx, cs, srs, h
+        if check and pk.vk_write(fmt) != head:
+            pk.close()
+            raise ZkbError("pk file: the vk commitments differ from the ones the key's values give")
+        return pk
+
     def close(self):
         # finalisers of garbage run in no fixed order (at interpreter exit a failed test's traceback can hold the last key): once
         # the context is destroyed the key's C state points into freed memory, so it is dropped, not destroyed
@@ -377,6 +436,83 @@ class ProvingKey:
     def __del__(self):
         try: self.close()
         except Exception: pass
+
+
+PK_SECTIONS = ("l0", "l_last", "l_active_row", "fixed_values", "fixed_polys", "fixed_cosets", "permutation values", "permutation polys",
+               "permutation cosets")
+PK_MISMATCH = 4         # ZKB_PK_MISMATCH; ZKB_SERDE_NON_CANONICAL = 2 is the other reason
+_IO_EOF = 1             # ZKB_IO_EOF
+PkReadReport = namedtuple("PkReadReport", "section column reason first_index count")   # zkb_pk_read_report
+
+
+class _PkReadReport(ctypes.Structure):
+    _fields_ = [("section", ctypes.c_uint32), ("column", ctypes.c_uint32), ("reason", ctypes.c_uint32), ("reserved", ctypes.c_uint32),
+                ("first_index", ctypes.c_uint64), ("count", ctypes.c_uint64)]
+
+
+_IO_READ = ctypes.CFUNCTYPE(ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint64)
+_IO_WRITE = ctypes.CFUNCTYPE(ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p, ctypes.c_uint64)
+
+
+class _IoVtable(ctypes.Structure):
+    _fields_ = [("user", ctypes.c_void_p), ("read", _IO_READ), ("write", _IO_WRITE)]
+
+
+@contextlib.contextmanager
+def _binary_file(path_or_file, mode):
+    if isinstance(path_or_file, (str, bytes, os.PathLike)):
+        with open(path_or_file, mode) as f:
+            yield f
+    else:
+        yield path_or_file
+
+
+def _read_exact(f, n, what):
+    data = f.read(n)
+    if len(data) != n:
+        raise ZkbError(f"pk file: the input ends inside {what}")
+    return data
+
+
+class _CallbackIo:
+    """zkb_io_vtable over a binary reader (readinto) or a writer callable: read_exact / write_all.  The writer gets a memoryview of
+    the library's buffer, valid only during the call (file.write and BytesIO.write copy it)."""
+
+    def __init__(self, reader=None, writer=None):
+        self.error = None
+
+        def rd(_user, buf, n):
+            try:
+                view = memoryview((ctypes.c_uint8 * n).from_address(buf)).cast("B")
+                got = 0
+                while got < n:
+                    r = reader.readinto(view[got:])
+                    if not r:
+                        return _IO_EOF
+                    got += r
+                return 0
+            except Exception as e:   # never let a Python exception unwind through C
+                self.error = e
+                return 2
+
+        def wr(_user, buf, n):
+            try:
+                writer(memoryview((ctypes.c_uint8 * n).from_address(buf)).cast("B") if n else b"")
+                return 0
+            except Exception as e:
+                self.error = e
+                return 2
+        self._keep = (_IO_READ(rd), _IO_WRITE(wr))
+        self.vt = _IoVtable(None, *self._keep)
+
+    def run(self, rc):
+        """check(rc), chaining the exception a callback raised"""
+        try:
+            check(rc)
+        except ZkbError as e:
+            if self.error is not None:
+                raise e from self.error
+            raise
 
 
 TRANSCRIPTS = {"blake2b": 0, "poseidon": 1, "evm": 2}
